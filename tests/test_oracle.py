@@ -170,3 +170,72 @@ def test_burgers_ide_disc_golden_both_oracles():
     assert 1e-14 < abs(f64 - float(g["loss2"])) / float(g["loss2"]) < 1e-8
     U0, U1 = pb.predict(g["w2"], g["x_star"])
     assert np.allclose(U0, g["predict_U0"], rtol=0, atol=1e-13) and np.allclose(U1, g["predict_U1"], rtol=0, atol=1e-13)
+
+
+def _golden_evaluations():
+    """(name, golden loss parts, parameter blocks, f(dtype, magnitudes) -> Taylor oracle result) on the golden inputs of
+    all five models."""
+    out = []
+    g = load_golden("burgers_inf")
+    L = [int(v) for v in g["layers"]]
+    out.append(("burgers_inf", g["parts"], ty.param_blocks(L),
+                lambda dt, m, g=g, L=L: ty.burgers_loss_grad(g["w"], L, g["lb"], g["ub"], g["X_f"], g["X_u"], g["u"],
+                                                             nu=float(g["nu"]), dtype=dt, magnitudes=m)))
+    g = load_golden("burgers_ide")
+    for wk in ("w", "w2"):
+        out.append(("burgers_ide_" + wk, g["parts"] if wk == "w" else None, ty.param_blocks(L, 2),
+                    lambda dt, m, g=g, wk=wk: ty.burgers_loss_grad(g[wk], L, g["lb"], g["ub"], None, g["X_u"], g["u"],
+                                                                   identification=True, dtype=dt, magnitudes=m)))
+    g = load_golden("nls_inf")
+    Ln = [int(v) for v in g["layers"]]
+    for tag, X0 in (("q1", g["x0"]), ("x0t0", np.concatenate([g["x0"], 0 * g["x0"]], 1))):
+        out.append(("nls_" + tag, g["parts_" + tag], ty.param_blocks(Ln),
+                    lambda dt, m, g=g, X0=X0: ty.schrodinger_loss_grad(g["w"], Ln, g["lb"], g["ub"], g["X_f"], g["tb"], X0,
+                                                                       g["uv0"], dtype=dt, magnitudes=m)))
+    g = load_golden("burgers_disc")
+    Ld = [int(v) for v in g["layers"]]
+    out.append(("burgers_disc", g["parts"], ty.param_blocks(Ld),
+                lambda dt, m, g=g: ty.burgers_disc_loss_grad(g["w"], Ld, g["lb"], g["ub"], g["x_0"], g["u_0"], g["x_1"],
+                                                             float(g["nu"]), float(g["dt"]), g["IRK"].astype(np.float64),
+                                                             dtype=dt, magnitudes=m)))
+    g = load_golden("burgers_ide_disc")
+    Le = [int(v) for v in g["layers"]]
+    for tag in ("", "2"):
+        out.append(("burgers_ide_disc" + tag, g["parts" + tag], ty.param_blocks(Le, 2),
+                    lambda dt, m, g=g, tag=tag: ty.burgers_ide_disc_loss_grad(g["w" + tag], Le, g["lb"], g["ub"], g["x_0"],
+                                                                              g["u_0"], g["x_1"], g["u_1"], float(g["dt"]),
+                                                                              g["IRK_alpha"], g["IRK_beta"], dtype=dt,
+                                                                              magnitudes=m)))
+    return out
+
+
+def test_float64_oracle_still_reproduces_the_golden_files_exactly():
+    """The dtype / magnitudes options leave the float64 arithmetic alone: the loss parts stored by make_golden.py (computed by
+    this oracle) come back bit for bit, and asking for the magnitudes does not change the gradient."""
+    for name, parts, blocks, f in _golden_evaluations():
+        loss, grad, pr = f(np.float64, False)
+        loss_m, grad_m, pr_m, mag = f(np.float64, True)
+        if parts is not None:
+            assert np.array_equal(np.array(pr, dtype=np.float64), np.asarray(parts)[:len(pr)]), name
+        assert loss_m == loss and np.array_equal(grad_m, grad) and np.array_equal(np.array(pr_m), np.array(pr)), name
+        assert grad.dtype == np.float64 and mag.shape == grad.shape and np.all(mag >= np.abs(grad) * (1 - 1e-12)), name
+        assert blocks[-1][1].stop == grad.size, name
+
+
+@pytest.mark.skipif(np.finfo(np.longdouble).eps > 1e-18, reason="np.longdouble has no extended precision on this platform")
+def test_longdouble_oracle_agrees_with_float64_per_block():
+    """The same sums in 64-bit-mantissa arithmetic.  At the golden (initialisation-scale) weights fp64 is good to ~1e-14 per
+    block, so the two must agree to 1e-13 on every W_l, b_l, lambda and loss part; a path that rounds to a narrower type would
+    not, and one that stays entirely in float64 fails the last check."""
+    for name, _, blocks, f in _golden_evaluations():
+        l64, g64, p64 = f(np.float64, False)
+        lld, gld, pld, mag = f(np.longdouble, True)
+        assert gld.dtype == np.longdouble and mag.dtype == np.longdouble, name
+        assert abs(l64 - lld) <= 1e-13 * abs(lld), name
+        for a, b in zip(p64, pld):
+            assert abs(a - b) <= 1e-13 * abs(b), name
+        for bn, sl in blocks:
+            err = np.linalg.norm((g64[sl] - gld[sl]).astype(np.longdouble))
+            assert err <= 1e-13 * np.linalg.norm(gld[sl]), (name, bn, float(err / np.linalg.norm(gld[sl])))
+        # ... and the extended precision is actually used: the two differ somewhere
+        assert not np.array_equal(g64, gld.astype(np.float64)), name
