@@ -166,7 +166,8 @@ int pinn_lbfgs_history(pinn_t* h, double* f_hist_out, int capacity, int* n_out);
  * and quirks.  Protocol:  create(x0) -> f,g = opfunc(x0) -> feed(f, g) -> while status == PINN_LBFGS_RUNNING:
  * f,g = opfunc(x_next); feed(f, g).  feed() returns in x_next the point to evaluate next or, once status != 0, the vector
  * lbfgs() returns; logged_iter >= 1 names the iteration the reference would have logged after this evaluation (with its f),
- * -1 none.  max_eval == 0 selects the reference default 1.25 * max_iter; n <= 32768. */
+ * -1 none.  max_eval == 0 selects the reference default 1.25 * max_iter.  The default (literal, single-CTA) kernel takes
+ * n <= 32768; with PINN_LBFGS=gram (Gram-matrix formulation) n may be larger, up to 2^30. */
 typedef struct pinn_lbfgs_handle pinn_lbfgs_t;
 int pinn_lbfgs_create(pinn_lbfgs_t** out, int device, int64_t n, const double* x0, int max_iter, double learning_rate,
                       int n_correction, double tol_fun, double tol_x, double max_eval);

@@ -387,14 +387,24 @@ def adam_init(P: int) -> AdamState:
 
 
 def adam_update(w: np.ndarray, g: np.ndarray, st: AdamState, lr: float, b1: float = 0.9, b2: float = 0.999,
-                eps: Optional[float] = None) -> np.ndarray:
+                eps: Optional[float] = None, dtype=np.float64) -> np.ndarray:
     """ResourceApplyAdam: alpha_t = lr*sqrt(1-b2^t)/(1-b1^t); m += (g-m)(1-b1); v += (g^2-v)(1-b2);
-    w -= alpha_t*m/(sqrt(v)+eps)   (eps outside the bias correction; eps None -> 1e-7)."""
+    w -= alpha_t*m/(sqrt(v)+eps)   (eps outside the bias correction; eps None -> 1e-7).
+
+    dtype=np.longdouble carries m, v, the bias correction and the update in that type (m and v are converted on first use);
+    the float64 path is the reference's arithmetic, unchanged."""
     eps = TF_KERAS_EPSILON if eps is None else eps
     st.t += 1
-    alpha = lr * math.sqrt(1.0 - b2 ** st.t) / (1.0 - b1 ** st.t)
-    st.m += (g - st.m) * (1.0 - b1)
-    st.v += (g * g - st.v) * (1.0 - b2)
+    if dtype is np.float64:
+        alpha = lr * math.sqrt(1.0 - b2 ** st.t) / (1.0 - b1 ** st.t)
+        c1, c2 = 1.0 - b1, 1.0 - b2
+    else:
+        one, b1, b2, eps = dtype(1), dtype(b1), dtype(b2), dtype(eps)
+        alpha = dtype(lr) * np.sqrt(one - b2 ** st.t) / (one - b1 ** st.t)
+        c1, c2 = one - b1, one - b2
+        st.m, st.v, g = st.m.astype(dtype, copy=False), st.v.astype(dtype, copy=False), np.asarray(g, dtype=dtype)
+    st.m += (g - st.m) * c1
+    st.v += (g * g - st.v) * c2
     return w - (st.m * alpha) / (np.sqrt(st.v) + eps)
 
 
@@ -430,6 +440,7 @@ class LbfgsTrace:
     d: List[np.ndarray] = field(default_factory=list)
     t: List[float] = field(default_factory=list)
     hist_len: List[int] = field(default_factory=list)
+    curv: List[Tuple[float, float]] = field(default_factory=list)   # (y.s, sum |y*s|) of the pair formed at iterations >= 2
     logged: List[Tuple[int, float]] = field(default_factory=list)
     stop_reason: str = ""
     n_iter: int = 0
@@ -437,20 +448,79 @@ class LbfgsTrace:
     x_final: Optional[np.ndarray] = None
 
 
+def _gram_direction(g: np.ndarray, S: List[np.ndarray], Y: List[np.ndarray], h_diag: float) -> Tuple[np.ndarray, float]:
+    """d and g.d of the Gram-matrix formulation of the two-loop recursion (csrc/optim_kernels.cuh lbfgs_solve / lbfgs_apply),
+    in float64 and in the kernels' association: the recurrences run in coefficient space over SY[a][b] = s_a.y_b and
+    YY[a][b] = y_a.y_b (ages, 0 = oldest), then d = c_g g + sum_m (ca_m s_m + cb_m y_m) and g.d from the same coefficients.
+    Mathematically the loop of lbfgs_fixed_step; the rounding differs, most where the stored pairs are nearly dependent."""
+    k = len(S)
+    Sm, Ym = np.array(S).reshape(k, g.size), np.array(Y).reshape(k, g.size)
+    SY, YY, sg, yg = Sm @ Ym.T, Ym @ Ym.T, Sm @ g, Ym @ g
+    ro = 1.0 / np.diag(SY)
+    al, acc = np.zeros(k), -sg                                     # first loop, newest to oldest
+    for j in range(k - 1, -1, -1):
+        al[j] = acc[j] * ro[j]
+        acc[:j] = acc[:j] - al[j] * SY[:j, j]
+    yq = -yg                                                       # y_i.q, q = -g - sum_m al_m y_m
+    for m in range(k):
+        yq = yq - al[m] * YY[:, m]
+    dl, acc = np.zeros(k), h_diag * yq                             # second loop, oldest to newest: dl_m = al_m - be_m
+    for m in range(k):
+        dl[m] = al[m] - acc[m] * ro[m]
+        acc[m + 1:] = acc[m + 1:] + dl[m] * SY[m, m + 1:]
+    cb = -h_diag * al
+    d = -h_diag * g
+    gtd = -h_diag * float(g @ g)
+    for m in range(k):
+        d = d + dl[m] * S[m]
+        d = d + cb[m] * Y[m]
+    for m in range(k):
+        gtd = gtd + cb[m] * yg[m]
+    for m in range(k):
+        gtd = gtd + dl[m] * sg[m]
+    return d, float(gtd)
+
+
+class ScriptedOpfunc(object):
+    """opfunc that returns recorded (f_k, g_k) in call order and ignores x: replays an optimiser on exactly the evaluations
+    another implementation saw.  Calling it more often than there are records is an error; ``assert_consumed`` checks the
+    replay asked for every record."""
+
+    def __init__(self, fs: Sequence[float], gs: Sequence[np.ndarray]):
+        assert len(fs) == len(gs)
+        self.fs, self.gs, self.calls = list(fs), list(gs), 0
+
+    def __call__(self, x):
+        assert self.calls < len(self.fs), "replay asked for evaluation %d of %d recorded" % (self.calls + 1, len(self.fs))
+        self.calls += 1
+        return self.fs[self.calls - 1], self.gs[self.calls - 1]
+
+    def assert_consumed(self):
+        assert self.calls == len(self.fs), "replay used %d of %d recorded evaluations" % (self.calls, len(self.fs))
+
+
 def lbfgs_fixed_step(opfunc: Callable[[np.ndarray], Tuple[float, np.ndarray]], x0: np.ndarray, max_iter: int,
                      learning_rate: float = 1.0, n_correction: int = 100, tol_fun: float = 1e-5,
-                     tol_x: float = 1e-19, max_eval: Optional[float] = None) -> Optional[LbfgsTrace]:
+                     tol_x: float = 1e-19, max_eval: Optional[float] = None, dtype=np.float64,
+                     direction: str = "literal") -> Optional[LbfgsTrace]:
     """Control flow of ``lbfgs`` with ``lineSearch`` unset (the only reachable configuration; the branch at
     custom_lbfgs.py:168-171 is dead).  Quirks kept: first step t=min(1,1/|g|_1) (:159-161); fixed step
     afterwards (:163); history only pushed when y.s > 1e-10 (:103) but the two-loop always runs (:116-141);
     `ro` recomputed from history each iteration (:121-123); no opfunc call after the last update (:176-182);
-    log after the stop tests (:217-221); returns None when maxIter == 0 (:43-44)."""
+    log after the stop tests (:217-221); returns None when maxIter == 0 (:43-44).
+
+    dtype=np.longdouble computes every vector, dot product and scalar in that type (the gradients are converted exactly).
+    direction="gram" (float64 only) replaces the two-loop recursion by its Gram-matrix formulation (_gram_direction)."""
+    assert direction in ("literal", "gram") and (direction == "literal" or dtype is np.float64)
     if max_iter == 0:
         return None
+    sc = float if dtype is np.float64 else dtype                   # scalars: Python floats on the reference's own path
     max_eval = max_eval or max_iter * 1.25                         # :49
     tr = LbfgsTrace()
-    x = np.array(x0, dtype=np.float64)
+    x = np.array(x0, dtype=dtype)
     f, g = opfunc(x)                                               # :65
+    if dtype is not np.float64:
+        g = np.asarray(g, dtype=dtype)
     tr.x_eval.append(x.copy()); tr.f_hist.append(f)
     n_eval = 1
     if np.sum(np.abs(g)) <= tol_fun:                               # :73-76
@@ -458,44 +528,52 @@ def lbfgs_fixed_step(opfunc: Callable[[np.ndarray], Tuple[float, np.ndarray]], x
         return tr
     S: List[np.ndarray] = []   # old_dirs (holds s = d*t)
     Y: List[np.ndarray] = []   # old_stps (holds y = g - g_old)
-    h_diag = 1.0
+    h_diag = sc(1.0)
     d = t = g_old = f_old = None
     n_iter = 0
     while n_iter < max_iter:                                       # :81
         n_iter += 1
+        gtd = None
         if n_iter == 1:                                            # :91-95
             d = -g
         else:
             y = g - g_old                                          # :98
             s = d * t                                              # :99
-            ys = float(np.sum(y * s))                              # :100
+            ys = sc(np.sum(y * s))                                 # :100
+            tr.curv.append((ys, sc(np.sum(np.abs(y * s)))))
             if ys > 1e-10:                                         # :102-114
                 if len(S) == n_correction:
                     S.pop(0); Y.pop(0)
                 S.append(s); Y.append(y)
-                h_diag = ys / float(np.sum(y * y))
+                h_diag = ys / sc(np.sum(y * y))
             k = len(S)
-            ro = [1.0 / float(np.sum(Y[i] * S[i])) for i in range(k)]     # :121-123
-            al = [0.0] * k
-            q = -g                                                 # :130
-            for i in range(k - 1, -1, -1):                         # :131-133
-                al[i] = float(np.sum(S[i] * q)) * ro[i]
-                q = q - al[i] * Y[i]
-            r = q * h_diag                                         # :136
-            for i in range(k):                                     # :137-139
-                be = float(np.sum(Y[i] * r)) * ro[i]
-                r = r + (al[i] - be) * S[i]
-            d = r
+            if direction == "gram":
+                d, gtd = _gram_direction(g, S, Y, h_diag)
+            else:
+                ro = [1.0 / sc(np.sum(Y[i] * S[i])) for i in range(k)]     # :121-123
+                al = [0.0] * k
+                q = -g                                             # :130
+                for i in range(k - 1, -1, -1):                     # :131-133
+                    al[i] = sc(np.sum(S[i] * q)) * ro[i]
+                    q = q - al[i] * Y[i]
+                r = q * h_diag                                     # :136
+                for i in range(k):                                 # :137-139
+                    be = sc(np.sum(Y[i] * r)) * ro[i]
+                    r = r + (al[i] - be) * S[i]
+                d = r
         g_old, f_old = g, f                                        # :144-145
-        gtd = float(np.sum(g * d))                                 # :151
+        if gtd is None:
+            gtd = sc(np.sum(g * d))                                # :151
         if gtd > -tol_x:                                           # :154-156
             tr.stop_reason = "no progress along direction"
             break
-        t = min(1.0, 1.0 / float(np.sum(np.abs(g)))) if n_iter == 1 else learning_rate    # :159-163
+        t = min(1.0, 1.0 / sc(np.sum(np.abs(g)))) if n_iter == 1 else learning_rate    # :159-163
         x = x + t * d                                              # :174
         tr.d.append(d.copy()); tr.t.append(t); tr.hist_len.append(len(S))
         if n_iter != max_iter:                                     # :176-182
             f, g = opfunc(x)
+            if dtype is not np.float64:
+                g = np.asarray(g, dtype=dtype)
             n_eval += 1
             tr.x_eval.append(x.copy()); tr.f_hist.append(f)
         if n_iter == max_iter:                                     # :192

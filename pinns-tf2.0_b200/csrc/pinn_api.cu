@@ -173,11 +173,10 @@ int disc_upload_points(pinn_t* h);
 // One L-BFGS iteration on the device (stop tests of the pending evaluation, history update, direction, step).
 // Default: the single-CTA kernel that follows the reference's loop literally (lbfgs_iterate).
 // PINN_LBFGS=gram selects the Gram-matrix formulation (lbfgs_dots -> lbfgs_solve -> lbfgs_apply: every SM reads its slice of
-// the history, so it takes less time per iteration).  It is NOT the default: in 1 of 8 long fixed-step runs (measured
-// with profiles/run_lbfgs_stability.py) its coefficient-space recursion produced a bad direction at iteration ~400 where the
-// literal loop did not -- the triangular recurrence over s_i.y_m amplifies rounding when the stored pairs are nearly
-// dependent, whereas the literal loop measures every s_i.q against the actual q -- and the reference has no line search to
-// recover from one bad step.
+// the history, so it takes less time per iteration, and it has no 32768-entry limit).  It is not the default: the literal
+// kernel is the reference's loop term by term.  Long fixed-step runs diverge from some starting points in BOTH modes
+// (profiles/lbfgs_stability_h100.jsonl); the step-by-step replay in tests/test_gpu_optimizer_replay.py keeps both kernels
+// within their fp64 error bound up to the divergence (DESIGN.md section 4.3).
 bool lbfgs_serial() {
   static int v = -1;
   if (v < 0) { const char* e = getenv("PINN_LBFGS"); v = (e && !strcmp(e, "gram")) ? 0 : 1; }

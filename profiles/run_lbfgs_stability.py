@@ -24,9 +24,7 @@ print(json.dumps({"adam_epochs": adam, "loss_after_adam": l_adam, "n_iter": r["n
 ''' % ROOT
 for mode in ("serial", "gram"):
     for adam in (100, 1900, 2000, 2100):
-        env = dict(os.environ)
-        if mode == "serial":
-            env["PINN_LBFGS"] = "serial"
+        env = dict(os.environ, PINN_LBFGS=mode)         # explicit for both: the serial kernel is the default
         r = subprocess.run([sys.executable, "-c", WORKER, str(adam), "3000"], env=env, capture_output=True, text=True, timeout=600)
         line = r.stdout.strip().splitlines()[-1] if r.stdout.strip() else json.dumps({"error": r.stderr[-300:]})
         print(json.dumps({"mode": mode, **json.loads(line)}), flush=True)

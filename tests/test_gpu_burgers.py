@@ -308,7 +308,7 @@ def test_quarter_million_point_shard(cabi):
 
 
 def test_gram_formulation_of_lbfgs_matches_the_literal_loop_on_short_runs():
-    """PINN_LBFGS=gram (opt-in; see pinn_api.cu: not the default because of a rare instability in LONG fixed-step runs): the golden
+    """PINN_LBFGS=gram (opt-in; see pinn_api.cu and DESIGN.md section 4.3): the golden
     6-iteration trace and a 60-iteration run with history overflow (n_corr = 7) against the default literal kernel."""
     import os
     import subprocess

@@ -124,6 +124,92 @@ def test_lbfgs_golden_trace():
     assert rel(tr.x_final, g["lbfgs_x_final"]) < 1e-9
 
 
+def _recorded(fn):
+    """fn wrapped so that every (f, g) it returns is kept, for a ScriptedOpfunc replay."""
+    fs, gs = [], []
+
+    def op(x):
+        f, g = fn(np.asarray(x, dtype=np.float64))
+        fs.append(f); gs.append(np.array(g, dtype=np.float64))
+        return f, g
+    return op, fs, gs
+
+
+def _steps_agree(a, b, tol):
+    """Worst per-iteration ||t a_d - t b_d|| / ||t b_d|| of two traces with the same control flow."""
+    assert a.stop_reason == b.stop_reason and a.n_iter == b.n_iter and a.n_eval == b.n_eval
+    assert a.logged == b.logged and a.hist_len == b.hist_len and len(a.d) == len(b.d)
+    worst = 0.0
+    for da, ta, db, tb in zip(a.d, a.t, b.d, b.t):
+        sa, sb = (np.asarray(ta * da, dtype=np.longdouble), np.asarray(tb * db, dtype=np.longdouble))
+        worst = max(worst, float(np.linalg.norm((sa - sb).astype(np.float64)) / np.linalg.norm(sb.astype(np.float64))))
+    assert worst <= tol, worst
+    return worst
+
+
+@pytest.mark.skipif(np.finfo(np.longdouble).eps > 1e-18, reason="np.longdouble has no extended precision on this platform")
+def test_lbfgs_longdouble_replay_agrees_with_float64_on_the_exit_objectives():
+    """The extended-precision L-BFGS replayed on the evaluations the float64 run saw (the objectives of
+    tests/test_gpu_lbfgs_foreign.py, which take every exit of the routine): same control flow, and every step t d within 1e-13
+    of the float64 one.  A replay that rounds to a narrower type would not agree; one left in float64 would agree exactly."""
+    from test_gpu_lbfgs_foreign import CASES
+    exact = 0
+    for name, fn, x0, reason, kw in CASES:
+        cfg = dict(max_iter=kw["maxIter"], learning_rate=kw.get("learningRate", 1.0), n_correction=kw.get("nCorrection", 100),
+                   tol_fun=kw.get("tolFun", 1e-5), tol_x=kw.get("tolX", 1e-19), max_eval=kw.get("maxEval"))
+        op, fs, gs = _recorded(fn)
+        tr64 = rp.lbfgs_fixed_step(op, np.asarray(x0, dtype=np.float64), **cfg)
+        assert tr64.stop_reason == reason, name
+        replay = rp.ScriptedOpfunc(fs, gs)
+        trld = rp.lbfgs_fixed_step(replay, np.asarray(x0, dtype=np.float64), dtype=np.longdouble, **cfg)
+        replay.assert_consumed()
+        assert all(d.dtype == np.longdouble for d in trld.d), name
+        _steps_agree(tr64, trld, 1e-13)
+        exact += all(np.array_equal(a, b.astype(np.float64)) for a, b in zip(tr64.d, trld.d))
+    assert exact < len(CASES)
+
+
+def test_lbfgs_gram_formulation_replay_agrees_with_the_literal_loop():
+    """The float64 Gram-matrix restatement of the device kernels (coefficient-space recurrences over s_a.y_b and y_a.y_b) against
+    the literal two-loop recursion on the same evaluations: 40 iterations with a 3-pair history (the ring wraps 12 times) on a
+    well-conditioned quadratic agree to 1e-12 per step; the two formulations round differently, so they are not identical."""
+    rng = np.random.default_rng(5)
+    M = rng.standard_normal((40, 40)); A = np.eye(40) + 0.3 * (M @ M.T) / 40; b = rng.standard_normal(40)
+    op, fs, gs = _recorded(_quad(A, b))
+    x0 = rng.standard_normal(40)
+    lit = rp.lbfgs_fixed_step(op, x0, max_iter=40, learning_rate=0.3, n_correction=3, tol_fun=1e-30)
+    assert lit.stop_reason == "max iterations" and max(lit.hist_len) == 3
+    replay = rp.ScriptedOpfunc(fs, gs)
+    gram = rp.lbfgs_fixed_step(replay, x0, max_iter=40, learning_rate=0.3, n_correction=3, tol_fun=1e-30, direction="gram")
+    replay.assert_consumed()
+    _steps_agree(lit, gram, 1e-12)
+    assert any(not np.array_equal(a, b) for a, b in zip(lit.d, gram.d))
+    with pytest.raises(AssertionError, match="recorded"):
+        replay(x0)
+
+
+@pytest.mark.skipif(np.finfo(np.longdouble).eps > 1e-18, reason="np.longdouble has no extended precision on this platform")
+def test_adam_longdouble_update_agrees_with_float64():
+    """Adam in extended precision from the same gradients: m, v and the bias correction carried in np.longdouble agree with the
+    float64 update, for the reference's hyperparameters and for eps-dominated and b1 = 0 ones.  The tolerance is set by float64
+    itself: 1 - b2^t cancels to about (1 - b2) t, so the bias correction of a float64 Adam is good to only ~1e-16 / ((1 - b2) t)
+    -- 1e-11 relative at b2 = 0.99999 and t = 1 -- while a float32 bias correction would be off by ~1e-7."""
+    rng = np.random.default_rng(1)
+    w0 = rng.standard_normal(500)
+    gs = [rng.standard_normal(500) * 10.0 ** rng.uniform(-6, 0, 500) for _ in range(30)]
+    for hp in (dict(lr=1e-3), dict(lr=0.05, b1=0.5, b2=0.9, eps=1e-2), dict(lr=1e-2, b1=0.0, b2=0.99999)):
+        s64, sld = rp.adam_init(500), rp.adam_init(500)
+        w = w0
+        for g in gs:
+            w64 = rp.adam_update(w, g, s64, **hp)
+            wld = rp.adam_update(w, g, sld, dtype=np.longdouble, **hp)
+            assert wld.dtype == np.longdouble and sld.m.dtype == np.longdouble
+            step = np.abs((wld - w).astype(np.float64))
+            assert np.all(np.abs((w64 - wld).astype(np.float64)) <= 1e-10 * step + np.spacing(np.abs(w64))), hp
+            w = w64
+        assert not np.array_equal(w64, wld.astype(np.float64)), hp
+
+
 def test_lua_struct_defaults_to_zero():
     s = rp.LuaStruct()
     s.maxIter = 3
