@@ -1,7 +1,10 @@
-// Fused Burgers PINN loss + gradient kernel, v2: warp-specialised (sm_90a, fp64 DMMA).
+// Fused Burgers PINN loss + gradient kernel, v2: warp-specialised (sm_90a, fp64 DMMA on Hopper's 16x8 shapes).
 //
-// Same mathematics and DMMA fragment scheme as burgers_fused.cuh (v1, kept as a cross-check), re-organised so that
-// the FP64 pipe of every SM sub-partition always has two warps to draw from and nobody waits at a block barrier:
+// Same mathematics as burgers_fused.cuh (v1, kept on m8n8k4 as a cross-check), re-organised so that the FP64 pipe of every
+// SM sub-partition always has two warps to draw from and nobody waits at a block barrier.  Its GEMMs run on DMMA.16x8x4
+// (chain) and DMMA.16x8x8 (weight gradient), which issue twice the FMAs per cycle of DMMA.8x8x4 on the H100
+// (profiles/microbench/fp64_peak_h100.jsonl).  Per 8-point tile: 210 DMMA.16x8x4 forward, 210 input adjoint and
+// 168 DMMA.16x8x8 weight gradient (v1: 420 + 420 + 504 DMMA.8x8x4).
 //
 //   warps 0-3  "chain" warps  : own an 8-point tile each; forward DMMA chain through the 8 tanh layers, residual,
 //                               seeds, then the backward chain (activation adjoints + input-adjoint DMMAs).  At
@@ -11,13 +14,11 @@
 //                               (a, a_x, a_t, a_xx) in [row][unit] layout, which is both what the division-free
 //                               backward formula needs and the A operand of the weight-gradient GEMM.
 //   warps 4-7  "wgrad" warps  : consume (stash[l-1], Z-bar_l) pairs of all four chain warps and run the
-//                               weight-gradient GEMM  G_l[i][j] += sum_rows H_{l-1}[row][i] Zbar_l[row][j]  with DMMA.
-//                               The 3x3 output tiles of a layer are OWNED by warps, a ROW of tiles each: position
-//                               k = (warp - layer) & 3 < 3 owns tiles (mt = k; nt = 0,1,2), position 3 takes one m-tile off
-//                               the busiest position at layers <= 3 and rests otherwise (ownership masks: 120/128/128/128
-//                               DMMAs per tile and warp; the roles rotate with the layer).  One A fragment
-//                               feeds up to three DMMAs, operand column pointers are chosen once per task (padded lanes point
-//                               into a ones/zeros page), so the unrolled k loop is 4 LDS + 3 DMMA without predicates.
+//                               weight-gradient GEMM  G_l[i][j] += sum_rows H_{l-1}[row][i] Zbar_l[row][j]  with DMMA.16x8x8
+//                               (M = 21 input rows incl. the bias ones-row, padded to 2 tiles of 16; N = 3 tiles of 8; K = the
+//                               32 staged rows).  The 42 output tiles of layers 1..7 are OWNED by warps, 11/11/10/10 (see
+//                               first_tile); operand column pointers are chosen once per task (padded lanes point into a
+//                               ones/zeros page), so the unrolled k loop has no predicates.
 //                               Accumulators live in registers for the whole kernel: no shared-memory accumulator, no
 //                               atomics, no cross-warp reduction, and a fixed summation order (deterministic results).
 //
@@ -28,6 +29,7 @@
 // the A-operand layout of k-step j of the next GEMM (the contraction index is permuted: k-step j contracts the units the
 // four lanes of a quad hold in slot j), so accumulators chain from layer to layer in registers, and the activation
 // arithmetic (tanh and the Taylor/adjoint formulas) runs on 5 instead of 6 values per lane -- no lane computes padding.
+// The m16n8k4 chain GEMMs stack two streams in one M = 16 tile (mma_layer5), whose fragment halves are these same layouts.
 //
 // Backward through a tanh layer in terms of its outputs (s = 1 - a^2; A* = adjoints of the outputs):
 //   Z_xx = s A_xx;  Z_t = s A_t;  Z_x = s A_x - 4 a a_x A_xx;
@@ -40,8 +42,8 @@
 // The tail of the evaluation runs in this launch too (optim_kernels.cuh: fused_tail): the last CTAs to finish reduce the per-CTA
 // partial vectors in a fixed order, exchange them with the other ranks over NVLink (multi-GPU) and apply Adam (Adam steps).
 //
-// Alternatives tried on the previous target GPU and dropped there as slower or equal (not re-measured on H100): 3-slot ring,
-// per-tile-pair ownership 3/2/2/2 instead of row ownership, holding the weight-gradient DMMAs back while the co-resident chain
+// Alternatives tried on the previous target GPU with DMMA.8x8x4 and dropped there as slower or equal (not re-measured on H100
+// or with the 16x8 shapes): 3-slot ring, holding the weight-gradient DMMAs back while the co-resident chain
 // warp is in a DMMA phase (the weight-gradient warps starve), publishing Z-bar after the chain warp's own input-adjoint GEMM,
 // output units 16..19 of the chain GEMMs (or columns 16..19 of the weight-gradient tile rows) as FMAs + a quad reduce-scatter
 // instead of the half-padded third DMMA tile (DFMA interleaved with DMMA costs more than it saves), spreading the
@@ -130,7 +132,8 @@ __device__ __forceinline__ void c_to_v5(double (&V)[4][5], const double (&Z)[4][
 }
 
 // Z[s][nt][:] += V_s * Bmat, Bmat[k][n] = Wl[k*ldk + n*ldn]  (forward: ldk = 20, ldn = 1; input adjoint: ldk = 1, ldn = 20,
-// i.e. the transposed weight).  N columns >= 20 read as zero.  5 k-steps x 4 streams x 3 N tiles = 60 DMMA.
+// i.e. the transposed weight).  N columns >= 20 read as zero.  Two streams share one M = 16 tile (stream 2p in rows 0..7,
+// stream 2p+1 in rows 8..15; the fragments are V5 and Z as they are): 5 k-steps x 2 stream pairs x 3 N tiles = 30 DMMA.16x8x4.
 __device__ __forceinline__ void mma_layer5(double (&Z)[4][3][2], const double (&V)[4][5], const double* Wl, int ldk, int ldn,
                                            int lane) {
   const int g = lane >> 2, q = lane & 3;
@@ -144,9 +147,9 @@ __device__ __forceinline__ void mma_layer5(double (&Z)[4][3][2], const double (&
       b[nt] = (n < W) ? Wl[k * ldk + n * ldn] : 0.0;
     }
 #pragma unroll
-    for (int s = 0; s < 4; s++)
+    for (int p = 0; p < 2; p++)
 #pragma unroll
-      for (int nt = 0; nt < 3; nt++) dmma(Z[s][nt], V[s][ks], b[nt]);
+      for (int nt = 0; nt < 3; nt++) dmma16x8x4(Z[2 * p][nt], Z[2 * p + 1][nt], V[2 * p][ks], V[2 * p + 1][ks], b[nt]);
   }
 }
 
@@ -213,52 +216,45 @@ __device__ __forceinline__ void load5(double (&V)[4][5], const double* T, int la
 // ---------------------------------------------------------------------------------------------------
 // wgrad warps
 // ---------------------------------------------------------------------------------------------------
-// tile-row ownership, hidden layers 1..7: position k = (wg - l) & 3; k < 3 owns row mt = k, k == 3 rests.  7 layers x 3 rows over
-// 4 warps is 6/5/5/5 rows (warp 3 rests only at layer 4); to level that, warp 3 hands the third N tile of its row at layers
-// 1, 2, 3 to the warp that rests there (warps 0, 1, 2): 120/128/128/128 DMMA per chain tile instead of 120/120/120/144.
-// mask: bit nt set = this warp accumulates tile (mt, nt).
-struct Own { int mt, mask; };
-__device__ __forceinline__ Own ownership(int l, int wg) {
-  const int k = (wg - l) & 3;
-  Own o;
-  if (k < 3) { o.mt = k; o.mask = (wg == 3 && l <= 3) ? 3 : 7; }
-  else if (l <= 3) { o.mt = (3 - l) & 3; o.mask = 4; }
-  else { o.mt = 0; o.mask = 0; }
-  return o;
-}
+// Output tiles of hidden layer l (1..7): G_l[i][j] (i = input unit 0..19 or 20 = the bias row, j = unit 0..19) is cut into
+// 2 M tiles of 16 (i = 0..15 | 16..20 + zero padding) x 3 N tiles of 8 (j = 0..7 | 8..15 | 16..19 + padding); tile t = 0..5
+// is (mt, nt) = (t & 1, t >> 1).  Tile t of layer l is number 6 (l - 1) + t of 42 and belongs to warp (6 (l - 1) + t) & 3:
+// the first tile of warp wg is t1 = (wg - 6 (l - 1)) & 3 and, for t1 < 2, the second is t1 + 4 (same M tile, N tile 2, so the
+// two share the A fragments).  Warps 0, 1 own two tiles at odd layers, warps 2, 3 at even layers: 11/11/10/10 tiles
+// (44/44/40/40 DMMA.16x8x8 per chain tile), one warp per output element, accumulated in a fixed order.
+__device__ __forceinline__ int first_tile(int l, int wg) { return (wg - 6 * (l - 1)) & 3; }
 
-// one weight-gradient task: accumulate this warp's tile row of layer L for one chain warp's 8-point tile.
-// Rows of the staged operands: R = 8*stream + 4*(ks&1) + q for k-step ks (K = 32 rows = 8 k-steps); A[row][i] = input unit i
-// of layer L (i == 20: the bias ones-row on the value stream), B[row][j] = Z-bar.
-template <int L, int MASK>
-__device__ __forceinline__ void wgrad_task(double (&acc)[3][2], int mt, const double* Aop, const double* ZB, const double* sm,
-                                           double sc0, double sc1, int lane) {
+// one weight-gradient task: accumulate this warp's tiles of layer L for one chain warp's 8-point tile.  K = the 32 staged
+// rows in 4 k-steps of 8: k-step st (= stream) contracts physical rows 8 st + q (k = q) and 8 st + 4 + q (k = q + 4), so a
+// quad's lanes read 4 rows 20 doubles apart and the stash and ring loads are bank-conflict-free with the prow() row order.  A[i][row] = output i of layer L-1 (i == 20:
+// the bias ones-row on the value stream), B[row][j] = Z-bar.  Operand pointers of padding rows and columns point into the
+// ones/zeros page, so the unrolled loop is 6 (TWO: 8) LDS + 1 (2) DMMA per k-step without predicates.
+template <bool TWO>
+__device__ __forceinline__ void wgrad_task(double (&c1)[2][2], double (&c2)[2][2], int t1, const double* Aop, const double* ZB,
+                                           const double* SP, int lane) {
   const int g = lane >> 2, q = lane & 3;
-  const double* SP = sm + SM_SPECIAL;
-  const double* Wsm = sm + SM_W;
-  const int i = 8 * mt + g;
-  const double* bp0 = ZB + g + q * W;
-  const double* bp1 = ZB + 8 + g + q * W;
-  const double* bp2 = (16 + g < W ? ZB + 16 + g : SP + 1) + q * W;
-  const double* ap = (i < W ? Aop + i : (i == W ? SP : SP + 1)) + q * W;          // [32 rows][W] outputs of layer L-1
+  const int mt = t1 & 1, nt = t1 >> 1;
+  auto acol = [&](int i) { return (i < W ? Aop + i : (i == W ? SP : SP + 1)) + q * W; };   // [32 rows][W] outputs of layer L-1
+  const double* ap0 = acol(16 * mt + g);
+  const double* ap1 = acol(16 * mt + 8 + g);
+  const double* bp1 = ZB + 8 * nt + g + q * W;                   // nt <= 1: a full N tile
+  const double* bp2 = (16 + g < W ? ZB + 16 + g : SP + 1) + q * W;   // the second tile is N tile 2
 #pragma unroll
-  for (int ks = 0; ks < 8; ks++) {
-    const int st = ks >> 1;
-    const int off = (8 * st + 4 * (ks & 1)) * W;              // physical row 8*stream + 4*(ks&1) (+ q, folded into the pointers)
-    const double a = ap[off];
-    if (MASK & 1) dmma(acc[0], a, bp0[off]);
-    if (MASK & 2) dmma(acc[1], a, bp1[off]);
-    if (MASK & 4) dmma(acc[2], a, bp2[off]);
+  for (int st = 0; st < 4; st++) {
+    const int off = 8 * st * W, off4 = off + 4 * W;
+    const double a0 = ap0[off], a1 = ap1[off], a2 = ap0[off4], a3 = ap1[off4];
+    dmma16x8x8(c1[0], c1[1], a0, a1, a2, a3, bp1[off], bp1[off4]);
+    if (TWO) dmma16x8x8(c2[0], c2[1], a0, a1, a2, a3, bp2[off], bp2[off4]);
   }
 }
 
 template <int L>
-__device__ __forceinline__ void wgrad_layer(double (&acc)[3][2], int wg, int it, int half, int cnt, const double* sm,
-                                            uint64_t* bars, double sc0, double sc1, int lane) {
+__device__ __forceinline__ void wgrad_layer(double (&c1)[2][2], double (&c2)[2][2], int wg, int it, int half, int cnt,
+                                            const double* sm, uint64_t* bars, int lane) {
   constexpr int J = 7 - L;                  // task index within a tile (layers 7..1)
   const int T = 7 * it + J;
   const int slot = T % RING;
-  const Own o = ownership(L, wg);
+  const int t1 = first_tile(L, wg);
 #pragma unroll 1
   for (int c = 2 * half; c < 2 * half + 2; c++) {
     if (4 * it + c >= cnt) break;           // chain warp c has no tile in this round (the CTA's last round may be partial)
@@ -266,10 +262,9 @@ __device__ __forceinline__ void wgrad_layer(double (&acc)[3][2], int wg, int it,
     const double* stash = sm + SM_STASH + c * STASH_PER_WARP;
     const double* Aop = stash + (L - 1) * STASHL;         // outputs of layer L-1 (STASH0 == STASHL)
     const double* ZB = sm + SM_RING + (c * RING + slot) * 640;
-    if (!PINN_ABL_NOWG) {                   // warp-uniform: the mask is a function of (layer, warp)
-      if (o.mask == 7) wgrad_task<L, 7>(acc, o.mt, Aop, ZB, sm, sc0, sc1, lane);
-      else if (o.mask == 3) wgrad_task<L, 3>(acc, o.mt, Aop, ZB, sm, sc0, sc1, lane);
-      else if (o.mask == 4) wgrad_task<L, 4>(acc, o.mt, Aop, ZB, sm, sc0, sc1, lane);
+    if (!PINN_ABL_NOWG) {                   // warp-uniform: t1 is a function of (layer, warp)
+      if (t1 < 2) wgrad_task<true>(c1, c2, t1, Aop, ZB, sm + SM_SPECIAL, lane);
+      else wgrad_task<false>(c1, c2, t1, Aop, ZB, sm + SM_SPECIAL, lane);
     }
     __syncwarp();
     if (lane == 0) mbar_arrive(bar_empty(bars, c, slot));
@@ -277,24 +272,30 @@ __device__ __forceinline__ void wgrad_layer(double (&acc)[3][2], int wg, int it,
 }
 
 template <int L>
-__device__ __forceinline__ void wgrad_flush(const double (&acc)[3][2], int wg, double* outp, int lane) {
+__device__ __forceinline__ void wgrad_flush_tile(const double (&acc)[2][2], int t, double* outp, int lane) {
   const int g = lane >> 2, q = lane & 3;
-  const Own o = ownership(L, wg);
-  const int in_dim = W;
-  const int i = 8 * o.mt + g;
+  const int mt = t & 1, nt = t >> 1;
 #pragma unroll
-  for (int nt = 0; nt < 3; nt++)
+  for (int h = 0; h < 2; h++)
 #pragma unroll
     for (int e = 0; e < 2; e++) {
-      const int j = 8 * nt + 2 * q + e;
-      if (j < W && ((o.mask >> nt) & 1)) {
-        if (i < in_dim) outp[woff(L) + i * W + j] = acc[nt][e];
-        else if (i == in_dim) outp[boff(L) + j] = acc[nt][e];
+      const int i = 16 * mt + 8 * h + g, j = 8 * nt + 2 * q + e;
+      if (j < W) {
+        if (i < W) outp[woff(L) + i * W + j] = acc[h][e];
+        else if (i == W) outp[boff(L) + j] = acc[h][e];
       }
     }
 }
+template <int L>
+__device__ __forceinline__ void wgrad_flush(const double (&c1)[2][2], const double (&c2)[2][2], int wg, double* outp, int lane) {
+  const int t1 = first_tile(L, wg);
+  wgrad_flush_tile<L>(c1, t1, outp, lane);
+  if (t1 < 2) wgrad_flush_tile<L>(c2, t1 + 4, outp, lane);
+}
 
-__global__ void __launch_bounds__(THREADS, 1) fused_loss_grad(const Args p) {
+// At most 252 registers so that the 8 warps fit the register file.  The 16x8 chain GEMMs take their A operand pairs and
+// accumulators in aligned register groups, and left alone ptxas uses 254; with the cap it fits without spills (ptxas -v).
+__global__ void __maxnreg__(252) fused_loss_grad(const Args p) {
   extern __shared__ __align__(16) double sm[];
   pdl_launch_dependents();                 // the tail kernel's blocks may be placed as SMs free up; they park in pdl_wait()
   if (p.run_flag && *p.run_flag != 0) return;
@@ -333,33 +334,37 @@ __global__ void __launch_bounds__(THREADS, 1) fused_loss_grad(const Args p) {
   if (warp >= CHAINS) {
     // =========================================== wgrad warps ===========================================
     const int wg = warp & 3;
-    double a1[3][2], a2[3][2], a3[3][2], a4[3][2], a5[3][2], a6[3][2], a7[3][2];
+    // first tile of each layer, and the second tiles: x[(L - 1) >> 1] is layer L's for warps 0, 1 (odd L) and 2, 3 (even L)
+    double a1[2][2], a2[2][2], a3[2][2], a4[2][2], a5[2][2], a6[2][2], a7[2][2], x[4][2][2];
 #pragma unroll
-    for (int s = 0; s < 3; s++)
+    for (int h = 0; h < 2; h++)
 #pragma unroll
-      for (int e = 0; e < 2; e++)
-        a1[s][e] = a2[s][e] = a3[s][e] = a4[s][e] = a5[s][e] = a6[s][e] = a7[s][e] = 0.0;
+      for (int e = 0; e < 2; e++) {
+        a1[h][e] = a2[h][e] = a3[h][e] = a4[h][e] = a5[h][e] = a6[h][e] = a7[h][e] = 0.0;
+#pragma unroll
+        for (int k = 0; k < 4; k++) x[k][h][e] = 0.0;
+      }
 #pragma unroll 1
     // The chain warps are consumed in two halves (chains 0,1 then chains 2,3).  Ring back-pressure then shifts the
     // halves by one phase: while one half runs its forward pass (which produces no weight-gradient work), the other
     // half runs its backward pass and keeps these warps -- and the FP64 pipe of every sub-partition -- busy.
     for (int it2 = 0; it2 < 2 * my_rounds; it2++) {
       const int it = it2 >> 1, half = it2 & 1;
-      wgrad_layer<7>(a7, wg, it, half, cnt, sm, bars, sc0, sc1, lane);
-      wgrad_layer<6>(a6, wg, it, half, cnt, sm, bars, sc0, sc1, lane);
-      wgrad_layer<5>(a5, wg, it, half, cnt, sm, bars, sc0, sc1, lane);
-      wgrad_layer<4>(a4, wg, it, half, cnt, sm, bars, sc0, sc1, lane);
-      wgrad_layer<3>(a3, wg, it, half, cnt, sm, bars, sc0, sc1, lane);
-      wgrad_layer<2>(a2, wg, it, half, cnt, sm, bars, sc0, sc1, lane);
-      wgrad_layer<1>(a1, wg, it, half, cnt, sm, bars, sc0, sc1, lane);
+      wgrad_layer<7>(a7, x[3], wg, it, half, cnt, sm, bars, lane);
+      wgrad_layer<6>(a6, x[2], wg, it, half, cnt, sm, bars, lane);
+      wgrad_layer<5>(a5, x[2], wg, it, half, cnt, sm, bars, lane);
+      wgrad_layer<4>(a4, x[1], wg, it, half, cnt, sm, bars, lane);
+      wgrad_layer<3>(a3, x[1], wg, it, half, cnt, sm, bars, lane);
+      wgrad_layer<2>(a2, x[0], wg, it, half, cnt, sm, bars, lane);
+      wgrad_layer<1>(a1, x[0], wg, it, half, cnt, sm, bars, lane);
     }
-    wgrad_flush<1>(a1, wg, outp, lane);
-    wgrad_flush<2>(a2, wg, outp, lane);
-    wgrad_flush<3>(a3, wg, outp, lane);
-    wgrad_flush<4>(a4, wg, outp, lane);
-    wgrad_flush<5>(a5, wg, outp, lane);
-    wgrad_flush<6>(a6, wg, outp, lane);
-    wgrad_flush<7>(a7, wg, outp, lane);
+    wgrad_flush<1>(a1, x[0], wg, outp, lane);
+    wgrad_flush<2>(a2, x[0], wg, outp, lane);
+    wgrad_flush<3>(a3, x[1], wg, outp, lane);
+    wgrad_flush<4>(a4, x[1], wg, outp, lane);
+    wgrad_flush<5>(a5, x[2], wg, outp, lane);
+    wgrad_flush<6>(a6, x[2], wg, outp, lane);
+    wgrad_flush<7>(a7, x[3], wg, outp, lane);
   } else {
     // =========================================== chain warps ===========================================
     const int c = warp;

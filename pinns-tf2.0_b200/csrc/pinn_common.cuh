@@ -14,6 +14,24 @@ __device__ __forceinline__ void dmma(double (&c)[2], double a, double b) {
                : "d"(a), "d"(b));
 }
 
+// ---- Hopper's 16x8 FP64 MMA shapes; SASS DMMA.16x8x4 / DMMA.16x8x8, native on sm_90a and twice the FMA rate of DMMA.8x8x4
+// there (profiles/microbench/fp64_peak_h100.jsonl).  The accumulator is two 8x8 halves laid out like the m8n8k4 C fragment:
+//   C/D: lo = [row g][cols 2q, 2q+1],  hi = [row g+8][cols 2q, 2q+1]
+// m16n8k4,  D(16x8) += A(16x4) * B(4x8):   a_lo = A[g][q], a_hi = A[g+8][q];   b = B[q][g]
+__device__ __forceinline__ void dmma16x8x4(double (&lo)[2], double (&hi)[2], double a_lo, double a_hi, double b) {
+  asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
+               : "+d"(lo[0]), "+d"(lo[1]), "+d"(hi[0]), "+d"(hi[1])
+               : "d"(a_lo), "d"(a_hi), "d"(b));
+}
+// m16n8k8,  D(16x8) += A(16x8) * B(8x8):   a0 = A[g][q], a1 = A[g+8][q], a2 = A[g][q+4], a3 = A[g+8][q+4];
+//                                          b0 = B[q][g], b1 = B[q+4][g]
+__device__ __forceinline__ void dmma16x8x8(double (&lo)[2], double (&hi)[2], double a0, double a1, double a2, double a3,
+                                           double b0, double b1) {
+  asm volatile("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+               : "+d"(lo[0]), "+d"(lo[1]), "+d"(hi[0]), "+d"(hi[1])
+               : "d"(a0), "d"(a1), "d"(a2), "d"(a3), "d"(b0), "d"(b1));
+}
+
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 // ---- mbarrier + TMA bulk copy (global -> shared, 1-D): SASS UBLKCP.  Used to stage the flat weight

@@ -1,5 +1,6 @@
 // FP64 pipe microbenchmark for H100 (sm_90a): DFMA peak, DMMA.8x8x4 peak, dependent-chain
-// latencies, and whether DFMA and DMMA issue concurrently.  Gives the roofline denominator for
+// latencies, and whether DFMA and DMMA issue concurrently; then the same for the 16x8 shapes
+// (DMMA.16x8x4/8/16) and a check of their fragment layouts.  Gives the roofline denominator for
 // the fused PINN kernels (MEASURED_PEAKS.json carries no FP64 figure).
 // Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o fp64_peak fp64_peak.cu
 #include <cstdio>
@@ -66,6 +67,111 @@ __global__ void mixed_kernel(double* out, int iters, double x) {
   out[blockIdx.x * blockDim.x + threadIdx.x] = s;
 }
 
+// ---- the Hopper FP64 MMA shapes.  S: 0 = m8n8k4, 1 = m16n8k4, 2 = m16n8k8, 3 = m16n8k16.  Fragments (lane = 4g + q):
+// A a_i = (row g + 8 (i & 1), col q + 4 (i >> 1)) for M = 16 (m8n8k4: a0 = (g, q)); B b_i = (row q + 4 i, col g);
+// C c_i = (row g + 8 (i >> 1), col 2q + (i & 1)).  layout_check() verifies these against a host GEMM.
+template <int S> struct Shape;
+template <> struct Shape<0> { static constexpr int M = 8, K = 4, NA = 1, NB = 1, NC = 2; static constexpr const char* name = "m8n8k4"; };
+template <> struct Shape<1> { static constexpr int M = 16, K = 4, NA = 2, NB = 1, NC = 4; static constexpr const char* name = "m16n8k4"; };
+template <> struct Shape<2> { static constexpr int M = 16, K = 8, NA = 4, NB = 2, NC = 4; static constexpr const char* name = "m16n8k8"; };
+template <> struct Shape<3> { static constexpr int M = 16, K = 16, NA = 8, NB = 4, NC = 4; static constexpr const char* name = "m16n8k16"; };
+
+template <int S>
+__device__ __forceinline__ void mma_s(double (&c)[4], const double (&a)[8], const double (&b)[4]) {
+  if (S == 0)
+    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
+                 : "+d"(c[0]), "+d"(c[1]) : "d"(a[0]), "d"(b[0]));
+  else if (S == 1)
+    asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
+                 : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3]) : "d"(a[0]), "d"(a[1]), "d"(b[0]));
+  else if (S == 2)
+    asm volatile("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+                 : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3]) : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(b[0]), "d"(b[1]));
+  else
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7,%8,%9,%10,%11}, "
+                 "{%12,%13,%14,%15}, {%0,%1,%2,%3};"
+                 : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+                 : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]),
+                   "d"(b[0]), "d"(b[1]), "d"(b[2]), "d"(b[3]));
+}
+
+template <int S, int ILP>
+__global__ void mma_kernel(double* out, int iters, double x) {
+  double c[ILP][4], a[8], b[4];
+#pragma unroll
+  for (int i = 0; i < ILP; i++) c[i][0] = c[i][1] = c[i][2] = c[i][3] = 0;
+#pragma unroll
+  for (int i = 0; i < 8; i++) a[i] = x * 1e-3 + threadIdx.x * 1e-12 + i * 1e-9;
+#pragma unroll
+  for (int i = 0; i < 4; i++) b[i] = x * 1e-3 + i * 1e-9;
+  for (int it = 0; it < iters; it++) {
+#pragma unroll
+    for (int i = 0; i < ILP; i++) mma_s<S>(c[i], a, b);
+  }
+  double s = 0;
+#pragma unroll
+  for (int i = 0; i < ILP; i++) s += c[i][0] + c[i][1] + c[i][2] + c[i][3];
+  out[blockIdx.x * blockDim.x + threadIdx.x] = s;
+}
+
+template <int S, int NM, int NF>
+__global__ void mixed_mma_kernel(double* out, int iters, double x) {
+  double c[NM + 1][4], a[8], b[4], f[NF + 1];
+#pragma unroll
+  for (int i = 0; i < NM; i++) c[i][0] = c[i][1] = c[i][2] = c[i][3] = 0;
+#pragma unroll
+  for (int i = 0; i < NF; i++) f[i] = i + threadIdx.x * 1e-9;
+#pragma unroll
+  for (int i = 0; i < 8; i++) a[i] = x * 1e-3 + threadIdx.x * 1e-12 + i * 1e-9;
+#pragma unroll
+  for (int i = 0; i < 4; i++) b[i] = x * 1e-3 + i * 1e-9;
+  for (int it = 0; it < iters; it++) {
+#pragma unroll
+    for (int i = 0; i < NM; i++) mma_s<S>(c[i], a, b);
+#pragma unroll
+    for (int i = 0; i < NF; i++) f[i] = fma(f[i], x, 1e-30);
+  }
+  double s = 0;
+#pragma unroll
+  for (int i = 0; i < NM; i++) s += c[i][0] + c[i][1] + c[i][2] + c[i][3];
+#pragma unroll
+  for (int i = 0; i < NF; i++) s += f[i];
+  out[blockIdx.x * blockDim.x + threadIdx.x] = s;
+}
+
+// one warp: C = A B with A[m][k] = m + 16 k + 1, B[k][n] = (k + 1) (n + 2) (exact in fp64), fragments as documented above
+template <int S>
+__global__ void layout_kernel(double* c_out) {
+  using Sh = Shape<S>;
+  const int g = threadIdx.x >> 2, q = threadIdx.x & 3;
+  double a[8] = {0, 0, 0, 0, 0, 0, 0, 0}, b[4] = {0, 0, 0, 0}, c[4] = {0, 0, 0, 0};
+  for (int i = 0; i < Sh::NA; i++) {
+    const int m = g + (Sh::M == 16 ? 8 * (i & 1) : 0), k = q + 4 * (Sh::M == 16 ? i >> 1 : i);
+    a[i] = m + 16 * k + 1;
+  }
+  for (int i = 0; i < Sh::NB; i++) b[i] = (q + 4 * i + 1) * (g + 2);
+  mma_s<S>(c, a, b);
+  for (int i = 0; i < Sh::NC; i++) c_out[(g + 8 * (i >> 1)) * 8 + 2 * q + (i & 1)] = c[i];
+}
+
+template <int S>
+int layout_check(double* dev) {
+  using Sh = Shape<S>;
+  CK(cudaMemset(dev, 0, 16 * 8 * sizeof(double)));
+  layout_kernel<S><<<1, 32>>>(dev);
+  double c[128];
+  CK(cudaMemcpy(c, dev, sizeof(c), cudaMemcpyDeviceToHost));
+  int bad = 0;
+  for (int m = 0; m < Sh::M; m++)
+    for (int n = 0; n < 8; n++) {
+      double r = 0;
+      for (int k = 0; k < Sh::K; k++) r += (double)(m + 16 * k + 1) * ((k + 1) * (n + 2));
+      bad += c[m * 8 + n] != r;
+    }
+  printf("{\"shape\": \"%s\", \"fragment_layout_ok\": %s}\n", Sh::name, bad ? "false" : "true");
+  return 0;
+}
+
 // FP32 FFMA for context
 template <int ILP>
 __global__ void ffma_kernel(float* out, int iters, float x) {
@@ -92,6 +198,46 @@ float time_ms(F launch, int reps = 5) {
     float ms; cudaEventElapsedTime(&ms, e0, e1); if (ms < best) best = ms;
   }
   return best;
+}
+
+// per shape: throughput at 1, 2 and 4 warps per sub-partition (ILP 8), the ILP sweep at one warp per sub-partition, and
+// the DMMA + DFMA mix.  "cyc_per_256fma" = issue cycles of one sub-partition per 256 FMAs (DMMA.8x8x4 = 1 instruction),
+// at the maximum SM clock.
+template <int S>
+int shape_sweep(int sms, int clk_khz, double* out) {
+  using Sh = Shape<S>;
+  const int iters = 4096;
+  const double fma_per_op = Sh::M * 8.0 * Sh::K;
+  const double cyc_per_ms = clk_khz;   // kHz = cycles per ms
+  for (int wpsp : {1, 2, 4}) {
+    const int grid = sms * 4, threads = 32 * wpsp;
+    float ms = time_ms([&] { mma_kernel<S, 8><<<grid, threads>>>(out, iters, 0.999); });
+    CK(cudaGetLastError());
+    const double ops_per_smsp = (double)wpsp * 8 * iters;
+    printf("{\"shape\": \"%s\", \"warps_per_smsp\": %d, \"tflops\": %.2f, \"cyc_per_op\": %.2f, \"cyc_per_256fma\": %.2f}\n", Sh::name,
+           wpsp, 2.0 * fma_per_op * ops_per_smsp * 4 * sms / ms / 1e9, ms * cyc_per_ms / ops_per_smsp,
+           ms * cyc_per_ms / ops_per_smsp * 256.0 / fma_per_op);
+  }
+  {
+    const int grid = sms * 4, threads = 32;
+    float m1 = time_ms([&] { mma_kernel<S, 1><<<grid, threads>>>(out, iters, 0.999); });
+    float m2 = time_ms([&] { mma_kernel<S, 2><<<grid, threads>>>(out, iters, 0.999); });
+    float m4 = time_ms([&] { mma_kernel<S, 4><<<grid, threads>>>(out, iters, 0.999); });
+    float m8 = time_ms([&] { mma_kernel<S, 8><<<grid, threads>>>(out, iters, 0.999); });
+    CK(cudaGetLastError());
+    printf("{\"shape\": \"%s\", \"one_warp_per_smsp\": true, \"cyc_per_op\": {\"ilp1\": %.2f, \"ilp2\": %.2f, \"ilp4\": %.2f, \"ilp8\": %.2f}}\n",
+           Sh::name, m1 * cyc_per_ms / iters, m2 * cyc_per_ms / iters / 2, m4 * cyc_per_ms / iters / 4, m8 * cyc_per_ms / iters / 8);
+  }
+  for (int wpsp : {1, 2}) {
+    const int grid = sms * 4, threads = 32 * wpsp;
+    float mm = time_ms([&] { mixed_mma_kernel<S, 8, 0><<<grid, threads>>>(out, iters, 0.999); });
+    float ff = time_ms([&] { mixed_mma_kernel<S, 0, 16><<<grid, threads>>>(out, iters, 0.999); });
+    float mf = time_ms([&] { mixed_mma_kernel<S, 8, 16><<<grid, threads>>>(out, iters, 0.999); });
+    CK(cudaGetLastError());
+    printf("{\"shape\": \"%s\", \"warps_per_smsp\": %d, \"ms_dmma8\": %.4f, \"ms_dfma16\": %.4f, \"ms_both\": %.4f, \"overlap\": %.2f}\n",
+           Sh::name, wpsp, mm, ff, mf, (mm + ff - mf) / (mm < ff ? mm : ff));
+  }
+  return 0;
 }
 
 int main() {
@@ -144,5 +290,9 @@ int main() {
     float ms = time_ms([&] { ffma_kernel<8><<<grid, threads>>>((float*)out, iters, 0.999f); });
     printf("{\"ffma_tflops\": %.2f}\n", 2.0 * grid * threads * 8.0 * iters / ms / 1e9);
   }
+  if (layout_check<0>(out) || layout_check<1>(out) || layout_check<2>(out) || layout_check<3>(out)) return 1;
+  if (shape_sweep<0>(sms, clk_khz, out) || shape_sweep<1>(sms, clk_khz, out) || shape_sweep<2>(sms, clk_khz, out) ||
+      shape_sweep<3>(sms, clk_khz, out))
+    return 1;
   return 0;
 }
