@@ -4,7 +4,7 @@
 // SM sub-partition always has two warps to draw from and nobody waits at a block barrier.  Its GEMMs run on DMMA.16x8x4
 // (chain) and DMMA.16x8x8 (weight gradient), which issue twice the FMAs per cycle of DMMA.8x8x4 on the H100
 // (profiles/microbench/fp64_peak_h100.jsonl).  Per 8-point tile: 210 DMMA.16x8x4 forward, 210 input adjoint and
-// 168 DMMA.16x8x8 weight gradient (v1: 420 + 420 + 504 DMMA.8x8x4).
+// 140 DMMA.16x8x8 weight gradient (v1: 420 + 420 + 504 DMMA.8x8x4).
 //
 //   warps 0-3  "chain" warps  : own an 8-point tile each; forward DMMA chain through the 8 tanh layers, residual,
 //                               seeds, then the backward chain (activation adjoints + input-adjoint DMMAs).  At
@@ -15,10 +15,10 @@
 //                               backward formula needs and the A operand of the weight-gradient GEMM.
 //   warps 4-7  "wgrad" warps  : consume (stash[l-1], Z-bar_l) pairs of all four chain warps and run the
 //                               weight-gradient GEMM  G_l[i][j] += sum_rows H_{l-1}[row][i] Zbar_l[row][j]  with DMMA.16x8x8
-//                               (M = 21 input rows incl. the bias ones-row, padded to 2 tiles of 16; N = 3 tiles of 8; K = the
-//                               32 staged rows).  The 42 output tiles of layers 1..7 are OWNED by warps, 11/11/10/10 (see
-//                               first_tile); operand column pointers are chosen once per task (padded lanes point into a
-//                               ones/zeros page), so the unrolled k loop has no predicates.
+//                               (G_l is 21 input rows incl. the bias ones-row x 20 units; 5 tiles of 16 x 8 per layer, one
+//                               of them transposed, see first_tile; K = the 32 staged rows).  The 35 output tiles of layers
+//                               1..7 are OWNED by warps, 9/9/9/8; operand column pointers are chosen once per task (padded
+//                               lanes point into a ones/zeros page), so the unrolled k loop has no predicates.
 //                               Accumulators live in registers for the whole kernel: no shared-memory accumulator, no
 //                               atomics, no cross-warp reduction, and a fixed summation order (deterministic results).
 //
@@ -87,6 +87,11 @@ constexpr int ROUND = CHAINS * TILE;      // 32 points per full CTA round
 #ifndef PINN_ABL_NODMMA
 #define PINN_ABL_NODMMA 0                 // no chain DMMAs
 #endif
+// phase profile (profiles/kernel_variants.py): every warp of CTAs 0 and 1 sums clock() deltas (SM cycles between issuing the
+// marks) per phase over one launch and printf's them at its end
+#ifndef PINN_PHASE_CLOCKS
+#define PINN_PHASE_CLOCKS 0
+#endif
 constexpr int RING = PINN_RING;           // Z-bar ring slots per chain warp
 
 // shared memory carve-up (doubles)
@@ -114,6 +119,24 @@ __device__ __forceinline__ uint64_t* bar_full(uint64_t* bars, int c, int slot) {
 __device__ __forceinline__ uint64_t* bar_empty(uint64_t* bars, int c, int slot) { return bars + 2 + (c * RING + slot) * 2; }
 __device__ __forceinline__ void wait_produced(uint64_t* bars, int c, int T) { mbar_wait(bar_full(bars, c, T % RING), (T / RING) & 1); }
 __device__ __forceinline__ void wait_consumed(uint64_t* bars, int c, int T) { mbar_wait(bar_empty(bars, c, T % RING), (T / RING) & 1); }
+
+// PINN_PHASE_CLOCKS: mark(k) adds the cycles since the previous mark to phase k.  Chain warps: forward GEMM, forward
+// elementwise (+ staging), output layer, backward elementwise (+ staging), backward GEMM, ring waits; weight-gradient warps:
+// DMMA tasks (phase 0), waits for Z-bar (phase 5).
+enum { PH_FWD_GEMM, PH_FWD_ACT, PH_OUT, PH_BWD_ACT, PH_BWD_GEMM, PH_WAIT, N_PHASES };
+struct PhaseClocks {
+#if PINN_PHASE_CLOCKS
+  unsigned acc[N_PHASES] = {}, t = (unsigned)clock();
+  __device__ __forceinline__ void mark(int k) { const unsigned n = (unsigned)clock(); acc[k] += n - t; t = n; }
+  __device__ __forceinline__ void report(int warp, int lane) const {
+    if (blockIdx.x < 2 && lane == 0)
+      printf("phase %d %d %u %u %u %u %u %u\n", blockIdx.x, warp, acc[0], acc[1], acc[2], acc[3], acc[4], acc[5]);
+  }
+#else
+  __device__ __forceinline__ void mark(int) {}
+  __device__ __forceinline__ void report(int, int) const {}
+#endif
+};
 
 // ---------------------------------------------------------------------------------------------------
 // chain warps: the V5 register layout
@@ -216,29 +239,33 @@ __device__ __forceinline__ void load5(double (&V)[4][5], const double* T, int la
 // ---------------------------------------------------------------------------------------------------
 // wgrad warps
 // ---------------------------------------------------------------------------------------------------
-// Output tiles of hidden layer l (1..7): G_l[i][j] (i = input unit 0..19 or 20 = the bias row, j = unit 0..19) is cut into
-// 2 M tiles of 16 (i = 0..15 | 16..20 + zero padding) x 3 N tiles of 8 (j = 0..7 | 8..15 | 16..19 + padding); tile t = 0..5
-// is (mt, nt) = (t & 1, t >> 1).  Tile t of layer l is number 6 (l - 1) + t of 42 and belongs to warp (6 (l - 1) + t) & 3:
-// the first tile of warp wg is t1 = (wg - 6 (l - 1)) & 3 and, for t1 < 2, the second is t1 + 4 (same M tile, N tile 2, so the
-// two share the A fragments).  Warps 0, 1 own two tiles at odd layers, warps 2, 3 at even layers: 11/11/10/10 tiles
-// (44/44/40/40 DMMA.16x8x8 per chain tile), one warp per output element, accumulated in a fixed order.
-__device__ __forceinline__ int first_tile(int l, int wg) { return (wg - 6 * (l - 1)) & 3; }
+// Output tiles of hidden layer l (1..7): G_l[i][j] (i = input unit 0..19 or 20 = the bias row, j = unit 0..19), 5 tiles:
+//   t = 0, 1, 4: rows i = 0..15 (M) x units j = 0..7 | 8..15 | 16..19 + padding (N tile nt = 0, 1, 2)
+//   t = 2:       TRANSPOSED, C[j][i] = G_l[i][j] for units j = 0..15 (M) x rows i = 16..23 (N: units 16..19, the bias row, padding)
+//   t = 3:       the corner, rows i = 16..20 + padding (M) x units j = 16..19 + padding (N)
+// Tile t of layer l is number 5 (l - 1) + t of 35 and belongs to warp (5 (l - 1) + t) & 3: the first tile of warp wg is
+// t1 = (wg - 5 (l - 1)) & 3 and, for t1 == 0, the second is tile 4 (same M tile as tile 0, so the two share the A fragments).
+// Warp wg owns two tiles at the layers l with l - 1 == wg (mod 4): 9/9/9/8 tiles (36/36/36/32 DMMA.16x8x8 per chain tile),
+// one warp per output element, accumulated in a fixed order.
+__device__ __forceinline__ int first_tile(int l, int wg) { return (wg - 5 * (l - 1)) & 3; }
 
 // one weight-gradient task: accumulate this warp's tiles of layer L for one chain warp's 8-point tile.  K = the 32 staged
 // rows in 4 k-steps of 8: k-step st (= stream) contracts physical rows 8 st + q (k = q) and 8 st + 4 + q (k = q + 4), so a
-// quad's lanes read 4 rows 20 doubles apart and the stash and ring loads are bank-conflict-free with the prow() row order.  A[i][row] = output i of layer L-1 (i == 20:
-// the bias ones-row on the value stream), B[row][j] = Z-bar.  Operand pointers of padding rows and columns point into the
-// ones/zeros page, so the unrolled loop is 6 (TWO: 8) LDS + 1 (2) DMMA per k-step without predicates.
+// quad's lanes read 4 rows 20 doubles apart and the stash and ring loads are bank-conflict-free with the prow() row order.
+// H[row][i] = output i of layer L-1 (i == 20: the bias ones-row on the value stream), Z[row][j] = Z-bar; the A operand is
+// H^T (Z-bar^T for the transposed tile t = 2), the B operand Z-bar (H).  Operand pointers of padding rows and columns point
+// into the ones/zeros page, so the unrolled loop is 6 (TWO: 8) LDS + 1 (2) DMMA per k-step without predicates.
 template <bool TWO>
 __device__ __forceinline__ void wgrad_task(double (&c1)[2][2], double (&c2)[2][2], int t1, const double* Aop, const double* ZB,
                                            const double* SP, int lane) {
   const int g = lane >> 2, q = lane & 3;
-  const int mt = t1 & 1, nt = t1 >> 1;
-  auto acol = [&](int i) { return (i < W ? Aop + i : (i == W ? SP : SP + 1)) + q * W; };   // [32 rows][W] outputs of layer L-1
-  const double* ap0 = acol(16 * mt + g);
-  const double* ap1 = acol(16 * mt + 8 + g);
-  const double* bp1 = ZB + 8 * nt + g + q * W;                   // nt <= 1: a full N tile
-  const double* bp2 = (16 + g < W ? ZB + 16 + g : SP + 1) + q * W;   // the second tile is N tile 2
+  auto hcol = [&](int i) { return (i < W ? Aop + i : (i == W ? SP : SP + 1)) + q * W; };   // [32 rows][W] outputs of layer L-1
+  auto zcol = [&](int j) { return (j < W ? ZB + j : SP + 1) + q * W; };                     // [32 rows][W] Z-bar
+  // tile t1: A rows (M) from ap0 (m = g) and ap1 (m = g + 8), B columns (N = g) from bp1; t1 == 0 with TWO: bp2 for tile 4
+  const double* ap0 = t1 == 2 ? zcol(g) : hcol(t1 == 3 ? 16 + g : g);
+  const double* ap1 = t1 == 2 ? zcol(8 + g) : hcol(t1 == 3 ? 24 + g : 8 + g);
+  const double* bp1 = t1 == 2 ? hcol(16 + g) : zcol(t1 == 3 ? 16 + g : 8 * t1 + g);
+  const double* bp2 = zcol(16 + g);
 #pragma unroll
   for (int st = 0; st < 4; st++) {
     const int off = 8 * st * W, off4 = off + 4 * W;
@@ -250,7 +277,7 @@ __device__ __forceinline__ void wgrad_task(double (&c1)[2][2], double (&c2)[2][2
 
 template <int L>
 __device__ __forceinline__ void wgrad_layer(double (&c1)[2][2], double (&c2)[2][2], int wg, int it, int half, int cnt,
-                                            const double* sm, uint64_t* bars, int lane) {
+                                            const double* sm, uint64_t* bars, int lane, PhaseClocks& pc) {
   constexpr int J = 7 - L;                  // task index within a tile (layers 7..1)
   const int T = 7 * it + J;
   const int slot = T % RING;
@@ -259,27 +286,30 @@ __device__ __forceinline__ void wgrad_layer(double (&c1)[2][2], double (&c2)[2][
   for (int c = 2 * half; c < 2 * half + 2; c++) {
     if (4 * it + c >= cnt) break;           // chain warp c has no tile in this round (the CTA's last round may be partial)
     wait_produced(bars, c, T);
+    pc.mark(PH_WAIT);
     const double* stash = sm + SM_STASH + c * STASH_PER_WARP;
     const double* Aop = stash + (L - 1) * STASHL;         // outputs of layer L-1 (STASH0 == STASHL)
     const double* ZB = sm + SM_RING + (c * RING + slot) * 640;
     if (!PINN_ABL_NOWG) {                   // warp-uniform: t1 is a function of (layer, warp)
-      if (t1 < 2) wgrad_task<true>(c1, c2, t1, Aop, ZB, sm + SM_SPECIAL, lane);
+      if (t1 == 0) wgrad_task<true>(c1, c2, t1, Aop, ZB, sm + SM_SPECIAL, lane);
       else wgrad_task<false>(c1, c2, t1, Aop, ZB, sm + SM_SPECIAL, lane);
     }
     __syncwarp();
     if (lane == 0) mbar_arrive(bar_empty(bars, c, slot));
+    pc.mark(PH_FWD_GEMM);
   }
 }
 
 template <int L>
 __device__ __forceinline__ void wgrad_flush_tile(const double (&acc)[2][2], int t, double* outp, int lane) {
   const int g = lane >> 2, q = lane & 3;
-  const int mt = t & 1, nt = t >> 1;
 #pragma unroll
   for (int h = 0; h < 2; h++)
 #pragma unroll
     for (int e = 0; e < 2; e++) {
-      const int i = 16 * mt + 8 * h + g, j = 8 * nt + 2 * q + e;
+      const int m = 8 * h + g, n = 2 * q + e;           // C[m][n] of the tile
+      const int i = t == 2 ? 16 + n : (t == 3 ? 16 + m : m);
+      const int j = t == 2 ? m : (t >= 3 ? 16 + n : 8 * t + n);
       if (j < W) {
         if (i < W) outp[woff(L) + i * W + j] = acc[h][e];
         else if (i == W) outp[boff(L) + j] = acc[h][e];
@@ -290,7 +320,7 @@ template <int L>
 __device__ __forceinline__ void wgrad_flush(const double (&c1)[2][2], const double (&c2)[2][2], int wg, double* outp, int lane) {
   const int t1 = first_tile(L, wg);
   wgrad_flush_tile<L>(c1, t1, outp, lane);
-  if (t1 < 2) wgrad_flush_tile<L>(c2, t1 + 4, outp, lane);
+  if (t1 == 0) wgrad_flush_tile<L>(c2, 4, outp, lane);
 }
 
 // At most 252 registers so that the 8 warps fit the register file.  The 16x8 chain GEMMs take their A operand pairs and
@@ -334,15 +364,16 @@ __global__ void __maxnreg__(252) fused_loss_grad(const Args p) {
   if (warp >= CHAINS) {
     // =========================================== wgrad warps ===========================================
     const int wg = warp & 3;
-    // first tile of each layer, and the second tiles: x[(L - 1) >> 1] is layer L's for warps 0, 1 (odd L) and 2, 3 (even L)
-    double a1[2][2], a2[2][2], a3[2][2], a4[2][2], a5[2][2], a6[2][2], a7[2][2], x[4][2][2];
+    PhaseClocks pc;
+    // first tile of each layer, and the second tiles: x[(L - 1) >> 2] is layer L's for warp L - 1 (layers 1..4) and L - 5 (5..7)
+    double a1[2][2], a2[2][2], a3[2][2], a4[2][2], a5[2][2], a6[2][2], a7[2][2], x[2][2][2];
 #pragma unroll
     for (int h = 0; h < 2; h++)
 #pragma unroll
       for (int e = 0; e < 2; e++) {
         a1[h][e] = a2[h][e] = a3[h][e] = a4[h][e] = a5[h][e] = a6[h][e] = a7[h][e] = 0.0;
 #pragma unroll
-        for (int k = 0; k < 4; k++) x[k][h][e] = 0.0;
+        for (int k = 0; k < 2; k++) x[k][h][e] = 0.0;
       }
 #pragma unroll 1
     // The chain warps are consumed in two halves (chains 0,1 then chains 2,3).  Ring back-pressure then shifts the
@@ -350,21 +381,22 @@ __global__ void __maxnreg__(252) fused_loss_grad(const Args p) {
     // half runs its backward pass and keeps these warps -- and the FP64 pipe of every sub-partition -- busy.
     for (int it2 = 0; it2 < 2 * my_rounds; it2++) {
       const int it = it2 >> 1, half = it2 & 1;
-      wgrad_layer<7>(a7, x[3], wg, it, half, cnt, sm, bars, lane);
-      wgrad_layer<6>(a6, x[2], wg, it, half, cnt, sm, bars, lane);
-      wgrad_layer<5>(a5, x[2], wg, it, half, cnt, sm, bars, lane);
-      wgrad_layer<4>(a4, x[1], wg, it, half, cnt, sm, bars, lane);
-      wgrad_layer<3>(a3, x[1], wg, it, half, cnt, sm, bars, lane);
-      wgrad_layer<2>(a2, x[0], wg, it, half, cnt, sm, bars, lane);
-      wgrad_layer<1>(a1, x[0], wg, it, half, cnt, sm, bars, lane);
+      wgrad_layer<7>(a7, x[1], wg, it, half, cnt, sm, bars, lane, pc);
+      wgrad_layer<6>(a6, x[1], wg, it, half, cnt, sm, bars, lane, pc);
+      wgrad_layer<5>(a5, x[1], wg, it, half, cnt, sm, bars, lane, pc);
+      wgrad_layer<4>(a4, x[0], wg, it, half, cnt, sm, bars, lane, pc);
+      wgrad_layer<3>(a3, x[0], wg, it, half, cnt, sm, bars, lane, pc);
+      wgrad_layer<2>(a2, x[0], wg, it, half, cnt, sm, bars, lane, pc);
+      wgrad_layer<1>(a1, x[0], wg, it, half, cnt, sm, bars, lane, pc);
     }
     wgrad_flush<1>(a1, x[0], wg, outp, lane);
     wgrad_flush<2>(a2, x[0], wg, outp, lane);
-    wgrad_flush<3>(a3, x[1], wg, outp, lane);
-    wgrad_flush<4>(a4, x[1], wg, outp, lane);
-    wgrad_flush<5>(a5, x[2], wg, outp, lane);
-    wgrad_flush<6>(a6, x[2], wg, outp, lane);
-    wgrad_flush<7>(a7, x[3], wg, outp, lane);
+    wgrad_flush<3>(a3, x[0], wg, outp, lane);
+    wgrad_flush<4>(a4, x[0], wg, outp, lane);
+    wgrad_flush<5>(a5, x[1], wg, outp, lane);
+    wgrad_flush<6>(a6, x[1], wg, outp, lane);
+    wgrad_flush<7>(a7, x[1], wg, outp, lane);
+    pc.report(warp, lane);
   } else {
     // =========================================== chain warps ===========================================
     const int c = warp;
@@ -394,6 +426,7 @@ __global__ void __maxnreg__(252) fused_loss_grad(const Args p) {
     };
     double xr_next = 0.0, tr_next = 0.0;
     if (n_tiles > 0) load_xt(0, xr_next, tr_next);
+    PhaseClocks pc;
 
 #pragma unroll 1
     for (int it = 0; it < n_tiles; it++) {
@@ -419,10 +452,13 @@ __global__ void __maxnreg__(252) fused_loss_grad(const Args p) {
         V[3][j] = 0.0;
       }
       act_forward5(V);
+      pc.mark(PH_FWD_ACT);
       // the stash is still the A operand of the previous tile's weight-gradient tasks: wait until its last one, the layer-1
       // task (J = 6), has been consumed; consumers retire tasks in order
       if (it > 0) wait_consumed(bars, c, 7 * (it - 1) + 6);
+      pc.mark(PH_WAIT);
       stage5(stash, V, lane);
+      pc.mark(PH_FWD_ACT);
       // ---------------- hidden layers 1..7: DMMA chain
 #pragma unroll 1
       for (int l = 1; l < NHID; l++) {
@@ -438,8 +474,10 @@ __global__ void __maxnreg__(252) fused_loss_grad(const Args p) {
           }
         if (!PINN_ABL_NODMMA) mma_layer5(Z, V, Wl, W, 1, lane);
         c_to_v5(V, Z, lane);
+        pc.mark(PH_FWD_GEMM);
         act_forward5(V);
         if (l < NHID - 1) stage5(stash + STASH0 + (l - 1) * STASHL, V, lane);
+        pc.mark(PH_FWD_ACT);
       }
       // ---------------- output layer (20 -> 1), residual, seeds
       double A[4][5];
@@ -487,16 +525,20 @@ __global__ void __maxnreg__(252) fused_loss_grad(const Args p) {
           g8[j] = acc;
         }
       }
+      pc.mark(PH_OUT);
       // ---------------- backward: layers 7..1 (task J = 7-l, ring slot J % RING)
 #pragma unroll 1
       for (int l = NHID - 1; l >= 1; l--) {
         const int T = 7 * it + (7 - l), slot = T % RING;
         if (l < NHID - 1) load5(V, stash + STASH0 + (l - 1) * STASHL, lane);        // outputs of layer l (l = 7: registers)
         act_backward5(A, V);                                                         // A := Z-bar
+        pc.mark(PH_BWD_ACT);
         if (T >= RING) wait_consumed(bars, c, T - RING);                             // the slot's previous task is done
+        pc.mark(PH_WAIT);
         stage5(sm + SM_RING + (c * RING + slot) * 640, A, lane);
         __syncwarp();
         if (lane == 0) mbar_arrive(bar_full(bars, c, slot));
+        pc.mark(PH_BWD_ACT);
         // adjoint of the layer inputs: A_new = Z-bar * W_l^T
         {
           const double* Wl = Wsm + woff(l);
@@ -508,6 +550,7 @@ __global__ void __maxnreg__(252) fused_loss_grad(const Args p) {
           if (!PINN_ABL_NODMMA) mma_layer5(An, A, Wl, 1, W, lane);
           c_to_v5(A, An, lane);
         }
+        pc.mark(PH_BWD_GEMM);
       }
       // ---------------- backward: layer 0: its weight gradient is 3 rows (x^, t^, bias) -- 25 FMAs per lane here instead of 24
       // DMMAs in a weight-gradient warp
@@ -521,6 +564,7 @@ __global__ void __maxnreg__(252) fused_loss_grad(const Args p) {
           g0b[j] += A[0][j];
         }
       }
+      pc.mark(PH_BWD_ACT);
     }
 
     // ---------------- chain-warp partials: losses, identification gradients, output-layer gradient
@@ -536,6 +580,7 @@ __global__ void __maxnreg__(252) fused_loss_grad(const Args p) {
       if (g == 0) { red[8 + u5[j]] = v; red[32 + u5[j]] = vx; red[32 + W + u5[j]] = vt; red[32 + 2 * W + u5[j]] = vb; }
     }
     if (lane == 0) { red[0] = loss_d; red[1] = loss_f; red[2] = gl1; red[3] = gl2; red[4] = gb8; }
+    pc.report(warp, lane);
   }
 
   __syncthreads();
