@@ -17,7 +17,7 @@
 // The reverse sweep needs the contraction over points (weight gradient), which is across lanes: Z-bar and the
 // layer inputs are transposed through a per-warp shared-memory staging area and fed to DMMA as a
 // [20(+1 ones row = bias) x 32 rows] x [32 rows x 20] GEMM.  Per-CTA accumulation is deterministic
-// (fixed warp order), the cross-CTA reduction is a second tiny kernel (reduce_partials).
+// (fixed warp order), the cross-CTA reduction is a second tiny kernel (reduce_tail).
 #pragma once
 #include "optim_kernels.cuh"
 
@@ -69,7 +69,7 @@ struct Args {
   double* partials;       // [gridDim.x][PSTRIDE]
   const int* run_flag;    // optional: skip the whole launch when *run_flag != 0 (L-BFGS stopped on device)
   int chains;             // unused (kept for ABI stability of the launch struct within this library)
-  FusedTail tail;         // v2, single-GPU Adam step: reduction + Adam by the last CTAs of this launch (optim_kernels.cuh)
+  Tail tail;              // v2: the evaluation's tail in the last CTAs of this launch (optim_kernels.cuh: fused_tail)
 };
 
 // ---------------------------------------------------------------------------------------------------

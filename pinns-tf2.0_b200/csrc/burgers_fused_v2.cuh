@@ -327,7 +327,6 @@ __device__ __forceinline__ void wgrad_flush(const double (&c1)[2][2], const doub
 // accumulators in aligned register groups, and left alone ptxas uses 254; with the cap it fits without spills (ptxas -v).
 __global__ void __maxnreg__(252) fused_loss_grad(const Args p) {
   extern __shared__ __align__(16) double sm[];
-  pdl_launch_dependents();                 // the tail kernel's blocks may be placed as SMs free up; they park in pdl_wait()
   if (p.run_flag && *p.run_flag != 0) return;
   double* Wsm = sm + SM_W;
   uint64_t* bars = reinterpret_cast<uint64_t*>(sm + SM_BAR);   // [0] weights TMA; then (full, empty) per (chain, slot)

@@ -129,7 +129,6 @@ __device__ __forceinline__ void block_reduce_store(double v, double* red, double
 __global__ void __launch_bounds__(THREADS, 2) fused_loss_grad(const Args p) {
   __shared__ double red[THREADS / 32];
   __shared__ int work_ctr;
-  pdl_launch_dependents();                 // the tail kernel's blocks may be placed as SMs free up; they park in pdl_wait()
   if (p.run_flag && *p.run_flag != 0) return;
   const int tid = threadIdx.x, lane = tid & 31;
   const int g = lane >> 2, q = lane & 3;

@@ -168,7 +168,6 @@ __device__ __forceinline__ void norm_coords(const Args& p, long long base, int n
 
 __global__ void __launch_bounds__(THREADS, 1) fused_loss_grad(const Args p) {
   extern __shared__ __align__(16) double sm[];
-  pdl_launch_dependents();                 // the tail kernel's blocks may be placed as SMs free up; they park in pdl_wait()
   if (p.run_flag && *p.run_flag != 0) return;
   double* Wsm = sm + SM_W;
   double* S0 = sm + SM_S0;

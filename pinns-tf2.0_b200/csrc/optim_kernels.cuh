@@ -64,18 +64,6 @@ __device__ __forceinline__ double reduce_block_entries(const double* __restrict_
   return combine8(red, lane);
 }
 
-__global__ void __launch_bounds__(256) reduce_partials(const double* __restrict__ partials, int n_cta, int stride,
-                                                       double* __restrict__ R, ReduceMap map, const int* __restrict__ run_flag) {
-  __shared__ double red[256];
-  pdl_wait();                                       // the fused kernel that wrote the partials has completed
-  if (run_flag && *run_flag != 0) return;
-  const int i = blockIdx.x * 32 + (threadIdx.x & 31);
-  const bool ok = i < map.n_out;
-  const int src = ok ? (i < map.p_net ? i : map.extra_src[i - map.p_net]) : 0;
-  const double s = reduce_block_entries(partials, n_cta, stride, src, ok, red);
-  if (ok && threadIdx.x < 32) R[i] = s;
-}
-
 // ------------------------------------------------------------------------------------------------
 // Adam (ResourceApplyAdam of TF 2.0):  alpha_t = lr sqrt(1-b2^t)/(1-b1^t); m += (g-m)(1-b1);
 // v += (g^2-v)(1-b2); w -= alpha_t m / (sqrt(v)+eps).   step[0] = t (completed steps).
@@ -90,62 +78,9 @@ __device__ __forceinline__ void adam_entry(double* w, double* m, double* v, doub
   w[i] -= (mi * alpha) / (sqrt(vi) + eps);
 }
 
-// step[0] = t (completed steps), step[1] = blocks finished in the current launch.  The LAST block to finish advances t,
-// so no block can observe the incremented counter (replaces a separate one-thread kernel).
-__device__ __forceinline__ void adam_finish(int* step, int nblocks) {
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    const int done = atomicAdd(step + 1, 1);
-    if (done == nblocks - 1) { step[1] = 0; step[0] += 1; __threadfence(); }
-  }
-}
-
-__global__ void adam_update(double* __restrict__ w, double* __restrict__ m, double* __restrict__ v,
-                            const double* __restrict__ R, int P, int* __restrict__ step, double lr, double b1, double b2,
-                            double eps, double* __restrict__ loss_ring, int ring) {
-  const int t = step[0] + 1;
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < P) adam_entry(w, m, v, R[i], i, t, lr, b1, b2, eps);
-  if (i == 0) loss_ring[(t - 1) % ring] = R[P] + R[P + 1] + R[P + 2];
-  adam_finish(step, gridDim.x);
-}
-
-// Single-GPU step: fixed-order reduction of the per-CTA partials fused with the Adam update (no collective between).
-__global__ void reduce_adam(const double* __restrict__ partials, int n_cta, int stride, double* __restrict__ R, ReduceMap map,
-                            double* __restrict__ w, double* __restrict__ m, double* __restrict__ v, int P,
-                            int* __restrict__ step, double lr, double b1, double b2, double eps,
-                            double* __restrict__ loss_ring, int ring) {
-  __shared__ double red[256];
-  pdl_wait();                                       // the fused kernel that wrote the partials has completed
-  const int t = step[0] + 1;
-  const int i = blockIdx.x * 32 + (threadIdx.x & 31);
-  const bool ok = i < map.n_out;
-  const int src = ok ? (i < map.p_net ? i : map.extra_src[i - map.p_net]) : 0;
-  const double s = reduce_block_entries(partials, n_cta, stride, src, ok, red);
-  if (ok && threadIdx.x < 32) {
-    R[i] = s;
-    if (i < P) adam_entry(w, m, v, s, i, t, lr, b1, b2, eps);
-  }
-  // the loss needs the three part sums, which live in (possibly) different blocks: the last block writes it
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    const int done = atomicAdd(step + 1, 1);
-    if (done == (int)gridDim.x - 1) {
-      __threadfence();
-      const volatile double* Rv = R;
-      loss_ring[(t - 1) % ring] = Rv[P] + Rv[P + 1] + Rv[P + 2];
-      step[1] = 0;
-      step[0] += 1;
-      __threadfence();
-    }
-  }
-}
-
 // ------------------------------------------------------------------------------------------------
-// Fused reduce -> all-to-all PUSH over NVLink peer memory -> (Adam) : ONE kernel per rank and evaluation (multi-GPU, one
-// process per GPU).  Replaces reduce_partials + ncclAllReduce + adam_update (3 launches + the NCCL kernel).
+// Reduce -> all-to-all PUSH over NVLink peer memory -> (Adam) in the tail of every evaluation (multi-GPU, one process per
+// GPU): one launch per rank and evaluation instead of a reduction + ncclAllReduce + adam_update.
 //
 // Every rank owns an IPC-exported exchange buffer   data[2 parities][world][slot_len] doubles, flag[2][world][n_blocks] u64.
 // Block b of rank r reduces its 32 entries of the per-CTA partials (fixed order), STORES them into slot [parity][r] of EVERY
@@ -235,71 +170,105 @@ __device__ __forceinline__ void exchange_block(int vb, const double* __restrict_
   }
 }
 
-// xseq[0] = published evaluations so far, xseq[1] = blocks finished in the current launch.
-// The grid is capped at a size that is certainly co-resident (the host passes min(n_vblocks, 2 x SMs)); every block walks
-// the 32-entry "virtual blocks" vb = blockIdx.x, blockIdx.x + gridDim.x, ... in increasing order.  A block waiting for the
-// peers' copy of vb therefore only depends on peers' blocks that wait for SMALLER virtual blocks: no cycle, whatever the order in
-// which the hardware dispatches blocks on the different GPUs.
-__global__ void __launch_bounds__(256)
-reduce_exchange(const double* __restrict__ partials, int n_cta, int stride, ReduceMap map, const int* __restrict__ run_flag,
-                XchgPeers peers, int* __restrict__ xseq, double* __restrict__ R, int* __restrict__ err, int adam,
-                double* __restrict__ w, double* __restrict__ m, double* __restrict__ v, int P, int* __restrict__ step,
-                double lr, double b1, double b2, double eps, double* __restrict__ loss_ring, int ring) {
-  pdl_wait();                                       // the fused kernel that wrote the partials has completed
-  if (run_flag && *run_flag != 0) return;          // identical on every rank (replicated L-BFGS state)
-  const unsigned long long seq = (unsigned long long)(*(volatile int*)xseq) + 1;
-  const int t = adam ? step[0] + 1 : 0;
-  const AdamDev ad{adam, w, m, v, P, t, lr, b1, b2, eps};
-  bool dead = false;
-  __shared__ double red[256], red2[256];
-  for (int vb = blockIdx.x; vb < peers.n_blocks; vb += gridDim.x)
-    exchange_block(vb, partials, n_cta, stride, map, peers, seq, err, R, ad, red, red2, dead);
+// ------------------------------------------------------------------------------------------------
+// The tail of an evaluation: the fixed-order reduction of the per-CTA partials into R = [grad | loss parts], 32 entries at a
+// time, with the exchange between ranks (world > 1, P2P) and the Adam update (Adam steps) in the same pass.  It runs either as
+// the stand-alone kernel reduce_tail or in the last CTAs of the fused loss/gradient launch (fused_tail); both run tail_block
+// and tail_finish, so the two forms give the same bits.
+// ------------------------------------------------------------------------------------------------
+struct Tail {
+  int enabled;            // fused kernels: run fused_tail at the end of the launch
+  double* R;
+  ReduceMap map;
+  int adam;               // 1: Adam step (update, loss ring, step counter); 0: evaluation only (L-BFGS, loss/gradient queries)
+  double *w, *m, *v;
+  int P;
+  double lr, b1, b2, eps;
+  double* loss_ring;
+  int ring;
+  int xchg;               // 1: exchange with the other ranks over peer memory
+  XchgPeers peers;
+  int* xseq;              // evaluations published to the peers so far (identical on all ranks)
+  int* err;               // raised when a peer never published
+  int* step;              // [0] completed Adam steps, [1] participants done, [2] fused_tail's tickets (both counters left at 0)
+};
+
+// One 32-entry block vb of R, executed by a whole block of 256 threads.  red: 512 doubles of shared memory.  t (the Adam step
+// being taken) and seq (the exchange's sequence number) are read once per participant by the caller: only tail_finish advances
+// them, after every participant's last block.
+__device__ __forceinline__ void tail_block(const Tail& tl, int vb, const double* __restrict__ partials, int n_cta, int stride,
+                                           double* red, int t, unsigned long long seq) {
+  const AdamDev ad{tl.adam, tl.w, tl.m, tl.v, tl.P, t, tl.lr, tl.b1, tl.b2, tl.eps};
+  if (tl.xchg) {
+    bool dead = false;                  // *err only ever goes from 0 to 1: the flag of one block is the flag of all later ones
+    exchange_block(vb, partials, n_cta, stride, tl.map, tl.peers, seq, tl.err, tl.R, ad, red, red + 256, dead);
+  } else {
+    const int i = vb * 32 + (threadIdx.x & 31);
+    const bool ok = i < tl.map.n_out;
+    const int src = ok ? (i < tl.map.p_net ? i : tl.map.extra_src[i - tl.map.p_net]) : 0;
+    const double s = reduce_block_entries(partials, n_cta, stride, src, ok, red);
+    if (ok && threadIdx.x < 32) {
+      tl.R[i] = s;
+      if (ad.on && i < ad.P) adam_entry(ad.w, ad.m, ad.v, s, i, t, ad.lr, ad.b1, ad.b2, ad.eps);
+    }
+  }
+  __syncthreads();                      // red is rewritten by the next block of entries
+}
+
+// Called by all threads of each of the n_part participants after its last block.  The last participant to finish writes the
+// loss (its three parts live in possibly different blocks) and advances the step to t, resets the counters and advances the
+// exchange sequence, so no participant can observe an advanced counter.
+__device__ __forceinline__ void tail_finish(const Tail& tl, int n_part, int t) {
   __threadfence();
   __syncthreads();
   if (threadIdx.x == 0) {
-    const int done = atomicAdd(xseq + 1, 1);
-    if (done == (int)gridDim.x - 1) {
+    const int done = atomicAdd(tl.step + 1, 1);
+    if (done == n_part - 1) {
       __threadfence();
-      if (adam && !dead) {
-        const volatile double* Rv = R;
-        loss_ring[(t - 1) % ring] = Rv[P] + Rv[P + 1] + Rv[P + 2];
-        step[0] += 1;
+      if (tl.adam && !(tl.xchg && *(volatile int*)tl.err != 0)) {     // a peer never published: optimiser state untouched
+        const volatile double* Rv = tl.R;
+        tl.loss_ring[(t - 1) % tl.ring] = Rv[tl.P] + Rv[tl.P + 1] + Rv[tl.P + 2];
+        *(volatile int*)tl.step = t;
       }
-      xseq[1] = 0;
-      xseq[0] += 1;
+      tl.step[1] = 0;
+      tl.step[2] = 0;
+      if (tl.xchg) *(volatile int*)tl.xseq = *(volatile int*)tl.xseq + 1;
       __threadfence();
     }
   }
 }
 
-// ------------------------------------------------------------------------------------------------
-// The tail INSIDE the fused loss/gradient launch (Adam steps with the specialised Burgers kernel): every CTA takes a ticket
-// after writing its partial vector; the last K to arrive (one per 32-entry block when the grid is large enough) wait for the
-// stragglers and then run the code of reduce_adam (one GPU) or of reduce_exchange (several: push exchange over NVLink) on
-// their blocks -- no second launch, no kernel boundary in the middle of a step.  Every CTA of the launch must be resident
-// (grid <= number of SMs, one CTA per SM), which holds for the persistent kernels that use it.  Same summation orders as the
-// stand-alone kernels: identical trajectories.  Across GPUs a tail CTA that waits for the peers' copy of block vb depends on
-// the peers' tail CTA that owns vb, which exists as soon as enough of the peer's CTAs have finished -- the peers' kernels run
-// to completion independently of the exchange, so there is no cycle.
-// ------------------------------------------------------------------------------------------------
-struct FusedTail {
-  int enabled;
-  int adam;               // 1: Adam step (update, loss ring, step counter); 0: evaluation only (L-BFGS, loss/gradient queries)
-  int* ctr;               // [0] CTAs that have written their partials, [1] tail CTAs that are done (both left at 0)
-  double* R;
-  ReduceMap map;
-  double *w, *m, *v;
-  int P;
-  int* step;
-  double lr, b1, b2, eps;
-  double* loss_ring;
-  int ring;
-  int xchg;               // world > 1: exchange over peer memory
-  XchgPeers peers;
-  int* xseq;
-  int* err;
-};
+// The stand-alone tail, one launch after the fused kernel.  With the exchange the grid is capped at a size that is certainly
+// co-resident (the host passes min(n_vblocks, 2 x SMs)); every block walks the 32-entry "virtual blocks" vb = blockIdx.x,
+// blockIdx.x + gridDim.x, ... in increasing order.  A block waiting for the peers' copy of vb therefore only depends on peers'
+// blocks that wait for SMALLER virtual blocks: no cycle, whatever the order in which the hardware dispatches blocks on the
+// different GPUs.
+__global__ void reduce_tail(const double* __restrict__ partials, int n_cta, int stride, const Tail tl, const int* __restrict__ run_flag) {
+  __shared__ double red[512];
+  if (run_flag && *run_flag != 0) return;          // identical on every rank (replicated L-BFGS state)
+  const int nb = (tl.map.n_out + 31) / 32;
+  const int t = tl.adam ? *(volatile int*)tl.step + 1 : 0;
+  const unsigned long long seq = tl.xchg ? (unsigned long long)(*(volatile int*)tl.xseq) + 1 : 0;
+  for (int vb = blockIdx.x; vb < nb; vb += gridDim.x) tail_block(tl, vb, partials, n_cta, stride, red, t, seq);
+  tail_finish(tl, gridDim.x, t);
+}
 
+// Adam on an R that is already complete (NCCL path: after the all-reduce).
+__global__ void adam_update(const Tail tl) {
+  const int t = tl.step[0] + 1;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < tl.P) adam_entry(tl.w, tl.m, tl.v, tl.R[i], i, t, tl.lr, tl.b1, tl.b2, tl.eps);
+  tail_finish(tl, gridDim.x, t);
+}
+
+// ------------------------------------------------------------------------------------------------
+// The tail INSIDE the fused loss/gradient launch (specialised Burgers kernel): every CTA takes a ticket after writing its
+// partial vector; the last K to arrive (one per 32-entry block when the grid is large enough) wait for the stragglers and then
+// run the tail on their blocks -- no second launch, no kernel boundary in the middle of a step.  Every CTA of the launch must
+// be resident (grid <= number of SMs, one CTA per SM), which holds for the persistent kernels that use it.  Across GPUs a tail
+// CTA that waits for the peers' copy of block vb depends on the peers' tail CTA that owns vb, which exists as soon as enough of
+// the peer's CTAs have finished -- the peers' kernels run to completion independently of the exchange, so there is no cycle.
+// ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ int ld_acquire_gpu(const int* p) {
   int v;
   asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
@@ -308,61 +277,27 @@ __device__ __forceinline__ int ld_acquire_gpu(const int* p) {
 
 // Called by ALL threads of every CTA after the CTA's partial vector has been written.  red: >= 512 doubles of shared memory
 // nobody else uses any more.
-__device__ __forceinline__ void fused_tail(const FusedTail& ft, const double* __restrict__ partials, int stride, double* red) {
+__device__ __forceinline__ void fused_tail(const Tail& tl, const double* __restrict__ partials, int stride, double* red) {
   __shared__ int s_slot;
-  const int nb = (ft.map.n_out + 31) / 32;
+  const int nb = (tl.map.n_out + 31) / 32;
   const int K = (int)gridDim.x < nb ? (int)gridDim.x : nb;            // tail CTAs: the last K to arrive
+  int* tickets = tl.step + 2;
   __threadfence();                                                    // this thread's partial entries, device-wide
   __syncthreads();
   if (threadIdx.x == 0) {
-    const int ticket = atomicAdd(ft.ctr, 1);
+    const int ticket = atomicAdd(tickets, 1);
     const int slot = ticket - ((int)gridDim.x - K);
     if (slot >= 0)
-      while (ld_acquire_gpu(ft.ctr) < (int)gridDim.x) __nanosleep(40);  // every partial vector is complete
+      while (ld_acquire_gpu(tickets) < (int)gridDim.x) __nanosleep(40);  // every partial vector is complete
     s_slot = slot;
   }
   __syncthreads();
   const int slot = s_slot;
   if (slot < 0) return;
-  const int t = ft.adam ? *(volatile int*)ft.step + 1 : 0;
-  bool dead = false;
-  if (ft.xchg) {
-    const unsigned long long seq = (unsigned long long)(*(volatile int*)ft.xseq) + 1;
-    const AdamDev ad{ft.adam, ft.w, ft.m, ft.v, ft.P, t, ft.lr, ft.b1, ft.b2, ft.eps};
-    for (int vb = slot; vb < nb; vb += K) {
-      exchange_block(vb, partials, (int)gridDim.x, stride, ft.map, ft.peers, seq, ft.err, ft.R, ad, red, red + 256, dead);
-      __syncthreads();                                                // red / red2 are rewritten by the next block of entries
-    }
-  } else {
-    for (int vb = slot; vb < nb; vb += K) {
-      const int i = vb * 32 + (threadIdx.x & 31);
-      const bool ok = i < ft.map.n_out;
-      const int src = ok ? (i < ft.map.p_net ? i : ft.map.extra_src[i - ft.map.p_net]) : 0;
-      const double s = reduce_block_entries(partials, (int)gridDim.x, stride, src, ok, red);
-      if (ok && threadIdx.x < 32) {
-        ft.R[i] = s;
-        if (ft.adam && i < ft.P) adam_entry(ft.w, ft.m, ft.v, s, i, t, ft.lr, ft.b1, ft.b2, ft.eps);
-      }
-      __syncthreads();                                                // red is rewritten by the next block of entries
-    }
-  }
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    const int done = atomicAdd(ft.ctr + 1, 1);
-    if (done == K - 1) {                                              // the last tail CTA: loss, step counter, counters back to 0
-      __threadfence();
-      if (ft.adam && !(ft.xchg && *(volatile int*)ft.err != 0)) {     // a peer never published: optimiser state untouched
-        const volatile double* Rv = ft.R;
-        ft.loss_ring[(t - 1) % ft.ring] = Rv[ft.P] + Rv[ft.P + 1] + Rv[ft.P + 2];
-        *(volatile int*)ft.step = t;
-      }
-      ft.ctr[0] = 0;
-      ft.ctr[1] = 0;
-      if (ft.xchg) *(volatile int*)ft.xseq = *(volatile int*)ft.xseq + 1;
-      __threadfence();
-    }
-  }
+  const int t = tl.adam ? *(volatile int*)tl.step + 1 : 0;
+  const unsigned long long seq = tl.xchg ? (unsigned long long)(*(volatile int*)tl.xseq) + 1 : 0;
+  for (int vb = slot; vb < nb; vb += K) tail_block(tl, vb, partials, (int)gridDim.x, stride, red, t, seq);
+  tail_finish(tl, K, t);
 }
 
 // ------------------------------------------------------------------------------------------------

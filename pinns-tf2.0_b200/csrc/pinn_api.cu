@@ -26,7 +26,7 @@ int fail(const std::string& m) { g_err = m; return -1; }
 // Live handles of this process.  A launch with the in-kernel tail (fused_tail) keeps its last CTAs spinning on their SMs until the
 // launch's stragglers arrive; two such launches running CONCURRENTLY on one device (two handles, two streams) could fill every SM
 // with spinning CTAs while both still have CTAs waiting for an SM.  So a handle uses the in-kernel tail only while no OTHER handle on
-// the same device has such a launch in flight (checked with cudaStreamQuery); otherwise it falls back to the tail kernels.
+// the same device has such a launch in flight (checked with cudaStreamQuery); otherwise it falls back to the tail kernel.
 std::mutex g_live_mu;
 std::vector<struct pinn_handle*> g_live;
 
@@ -143,12 +143,12 @@ struct pinn_handle {
   long long px_cap = 0, pout_cap = 0;
 
   ncclComm_t comm = nullptr;
-  // fused NVLink push exchange (optim_kernels.cuh: reduce_exchange)
+  // NVLink push exchange in the tail of every evaluation (optim_kernels.cuh: exchange_block)
   double* d_xchg = nullptr;            // [2][world][slot_len] doubles, then [2][world][n_blocks] u64 flags (IPC-exported)
   bool p2p_ready = false, p2p_mapped = false;
   pinn::XchgPeers peers{};
   void* peer_base[pinn::P2P_MAX] = {nullptr};
-  int* d_xseq = nullptr;               // [0] published evaluations, [1] block counter
+  int* d_xseq = nullptr;               // evaluations published to the peers
   int* d_p2p_err = nullptr;
 };
 
@@ -294,67 +294,44 @@ int ensure_points(pinn_t* h, long long need_d, long long need_c) {
 
 struct AdamArgs { double lr, b1, b2, eps; };
 
-// Launch a tail kernel, optionally with programmatic stream serialization (PDL, PINN_PDL=1): its blocks may then be placed while
-// the fused kernel that precedes it in the stream drains, and wait in pdl_wait() for its completion.  OFF by default: the
-// early-placed tail blocks sit on the SMs whose fused CTA finished first, and the launch latency they hide is small (it made the
-// step slower on the previous target GPU; not measured on H100).
-bool use_pdl() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("PINN_PDL"); v = (e && e[0] == '1') ? 1 : 0; }
-  return v == 1;
-}
-template <typename... KArgs, typename... Args>
-cudaError_t launch_tail_kernel(void (*kernel)(KArgs...), int grid, int block, cudaStream_t stream, Args... args) {
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3((unsigned)block); cfg.dynamicSmemBytes = 0; cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = use_pdl() ? 1 : 0;
-  cfg.attrs = attr; cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+// The tail of h's most recent fused launch (h->last_map): with Adam when ad != nullptr, with the P2P exchange when world > 1 and
+// the peers are connected.
+int make_tail(pinn_t* h, const AdamArgs* ad, pinn::Tail* tl) {
+  *tl = pinn::Tail{};
+  tl->R = h->d_R; tl->map = h->last_map; tl->step = h->d_step;
+  tl->w = h->d_w; tl->m = h->d_m; tl->v = h->d_v; tl->P = h->P;
+  tl->loss_ring = h->d_loss_ring; tl->ring = LOSS_RING;
+  if (ad) { tl->adam = 1; tl->lr = ad->lr; tl->b1 = ad->b1; tl->b2 = ad->b2; tl->eps = ad->eps; }
+  if (h->world > 1 && h->p2p_ready) {
+    if ((tl->map.n_out + 31) / 32 != h->peers.n_blocks || tl->map.n_out > h->peers.slot_len)
+      return fail("internal: exchange buffer geometry mismatch");
+    tl->xchg = 1; tl->peers = h->peers; tl->xseq = h->d_xseq; tl->err = h->d_p2p_err;
+  }
+  return 0;
 }
 
 // The tail of an evaluation: fixed-order reduction of the per-CTA partials into R = [grad | loss parts] on every rank,
 // optionally fused with the Adam update.
 // (Evaluations of the specialised Burgers kernel do all of this in their own last CTAs -- fused_tail -- and never get here.)
-//   world == 1      : reduce_partials, or reduce_adam (one kernel)
-//   world > 1, P2P  : reduce_exchange -- reduction + NVLink all-to-all push + rank-ordered sum (+ Adam) in ONE kernel
-//   world > 1, NCCL : reduce_partials + ncclAllReduce(P+3 doubles) (+ adam_update)
+//   world == 1, or P2P : reduce_tail -- reduction (+ NVLink all-to-all push + rank-ordered sum) (+ Adam) in ONE kernel
+//   world > 1, NCCL    : reduce_tail + ncclAllReduce(P+3 doubles) (+ adam_update)
 int launch_tail(pinn_t* h, const int* run_flag, const AdamArgs* ad) {
-  const pinn::ReduceMap& map = h->last_map;
-  const int nb = (map.n_out + 31) / 32;
-  if (h->world == 1) {
-    if (ad)
-      CUDA_TRY(launch_tail_kernel(pinn::reduce_adam, nb, 256, h->stream, h->d_partials, h->last_grid, h->last_stride, h->d_R, map, h->d_w,
-                                  h->d_m, h->d_v, h->P, h->d_step, ad->lr, ad->b1, ad->b2, ad->eps, h->d_loss_ring, LOSS_RING));
-    else
-      CUDA_TRY(launch_tail_kernel(pinn::reduce_partials, nb, 256, h->stream, h->d_partials, h->last_grid, h->last_stride, h->d_R, map,
-                                  run_flag));
-    CUDA_TRY(cudaGetLastError());
-    h->launches++;
-    return 0;
-  }
-  if (h->p2p_ready) {
-    if (nb != h->peers.n_blocks || map.n_out > h->peers.slot_len) return fail("internal: exchange buffer geometry mismatch");
-    const int xgrid = nb < 2 * h->n_sm ? nb : 2 * h->n_sm;      // certainly co-resident: <= 2 blocks of 256 threads per SM
-    CUDA_TRY(launch_tail_kernel(pinn::reduce_exchange, xgrid, 256, h->stream, h->d_partials, h->last_grid, h->last_stride, map, run_flag,
-                                h->peers, h->d_xseq, h->d_R, h->d_p2p_err, ad ? 1 : 0, h->d_w, h->d_m, h->d_v, h->P, h->d_step,
-                                ad ? ad->lr : 0.0, ad ? ad->b1 : 0.0, ad ? ad->b2 : 0.0, ad ? ad->eps : 0.0, h->d_loss_ring,
-                                LOSS_RING));
-    CUDA_TRY(cudaGetLastError());
-    h->launches++;
-    return 0;
-  }
-  CUDA_TRY(launch_tail_kernel(pinn::reduce_partials, nb, 256, h->stream, h->d_partials, h->last_grid, h->last_stride, h->d_R, map, run_flag));
+  const bool nccl = h->world > 1 && !h->p2p_ready;
+  pinn::Tail tl;
+  if (make_tail(h, nccl ? nullptr : ad, &tl)) return -1;
+  const int nb = (tl.map.n_out + 31) / 32;
+  const int grid = tl.xchg && nb > 2 * h->n_sm ? 2 * h->n_sm : nb;   // certainly co-resident: <= 2 blocks of 256 threads per SM
+  pinn::reduce_tail<<<grid, 256, 0, h->stream>>>(h->d_partials, h->last_grid, h->last_stride, tl, run_flag);
   CUDA_TRY(cudaGetLastError());
   h->launches++;
+  if (!nccl) return 0;
   // one exchange over [gradient | loss parts] (SURVEY 8(e)).  A skipped evaluation (L-BFGS stopped) still takes part with
   // stale but rank-identical participation so that ranks never diverge.
   int rc = g_nccl.AllReduce(h->d_R, h->d_R, (size_t)h->P + 3, NCCL_FLOAT64, NCCL_SUM, h->comm, h->stream);
   if (rc != 0) return fail(std::string("ncclAllReduce: ") + (g_nccl.GetErrorString ? g_nccl.GetErrorString(rc) : "error"));
   if (ad) {
-    pinn::adam_update<<<(h->P + 127) / 128, 128, 0, h->stream>>>(h->d_w, h->d_m, h->d_v, h->d_R, h->P, h->d_step, ad->lr, ad->b1,
-                                                                   ad->b2, ad->eps, h->d_loss_ring, LOSS_RING);
+    if (make_tail(h, ad, &tl)) return -1;
+    pinn::adam_update<<<(h->P + 127) / 128, 128, 0, h->stream>>>(tl);
     CUDA_TRY(cudaGetLastError());
     h->launches++;
   }
@@ -374,7 +351,7 @@ bool tail_slot_free(pinn_t* h) {
 }
 
 // v2 kernel with tail_done != nullptr: the launch also reduces the partials (+ exchanges them, + applies Adam when ad != nullptr) in
-// its last CTAs (fused_tail); *tail_done tells the caller that no tail kernel is needed.  PINN_FUSED_TAIL=0 keeps the tail kernels.
+// its last CTAs (fused_tail); *tail_done tells the caller that no tail kernel is needed.  PINN_FUSED_TAIL=0 keeps the tail kernel.
 int burgers_launch_eval(pinn_t* h, const int* run_flag, const AdamArgs* ad = nullptr, bool* tail_done = nullptr) {
   namespace B = pinn::burgers;
   const bool ide = h->pde == PINN_BURGERS_IDE;
@@ -412,18 +389,14 @@ int burgers_launch_eval(pinn_t* h, const int* run_flag, const AdamArgs* ad = nul
   map.extra_src[map.n_extra++] = 3023;        // (boundary part: always 0 for Burgers)
   map.extra_src[map.n_extra++] = B::IDX_LF;
   map.n_out = map.p_net + map.n_extra;
+  h->last_map = map; h->last_grid = grid; h->last_stride = B::PSTRIDE;
   static const bool fused_tail_on = [] { const char* e = getenv("PINN_FUSED_TAIL"); return !(e && e[0] == '0'); }();
-  const bool xchg_ok = h->world > 1 && h->p2p_ready && (map.n_out + 31) / 32 == h->peers.n_blocks && map.n_out <= h->peers.slot_len;
   // every evaluation of the v2 kernel carries its own tail: Adam steps (ad != nullptr) and plain evaluations (L-BFGS, loss/gradient
-  // queries; a launch skipped through run_flag skips its tail with it, exactly like the stand-alone tail kernels)
-  if (tail_done && fused_tail_on && (h->world == 1 || xchg_ok) && h->burgers_kernel == 2 && grid <= h->n_sm && tail_slot_free(h)) {
+  // queries; a launch skipped through run_flag skips its tail with it, exactly like the stand-alone tail kernel)
+  if (tail_done && fused_tail_on && (h->world == 1 || h->p2p_ready) && h->burgers_kernel == 2 && grid <= h->n_sm && tail_slot_free(h)) {
+    if (make_tail(h, ad, &a.tail)) return -1;
+    a.tail.enabled = 1;
     h->tail_inflight = true;
-    pinn::FusedTail& ft = a.tail;
-    ft.enabled = 1; ft.adam = ad ? 1 : 0; ft.ctr = h->d_step + 2; ft.R = h->d_R; ft.map = map;
-    if (h->world > 1) { ft.xchg = 1; ft.peers = h->peers; ft.xseq = h->d_xseq; ft.err = h->d_p2p_err; }
-    ft.w = h->d_w; ft.m = h->d_m; ft.v = h->d_v; ft.P = h->P; ft.step = h->d_step;
-    if (ad) { ft.lr = ad->lr; ft.b1 = ad->b1; ft.b2 = ad->b2; ft.eps = ad->eps; }
-    ft.loss_ring = h->d_loss_ring; ft.ring = LOSS_RING;
     *tail_done = true;
   }
   if (h->burgers_kernel == 2)
@@ -432,7 +405,6 @@ int burgers_launch_eval(pinn_t* h, const int* run_flag, const AdamArgs* ad = nul
     B::fused_loss_grad<<<grid, B::THREADS, B::SMEM_BYTES, h->stream>>>(a);
   CUDA_TRY(cudaGetLastError());
   h->launches++;
-  h->last_map = map; h->last_grid = grid; h->last_stride = B::PSTRIDE;
   return 0;
 }
 
@@ -620,8 +592,8 @@ int pinn_p2p_export(pinn_t* h, void* out64) {
     CUDA_TRY(cudaMemset(h->d_xchg, 0, data_bytes + flag_bytes));
     CUDA_TRY(cudaMalloc((void**)&h->d_p2p_err, 4));
     CUDA_TRY(cudaMemset(h->d_p2p_err, 0, 4));
-    CUDA_TRY(cudaMalloc((void**)&h->d_xseq, 8));
-    CUDA_TRY(cudaMemset(h->d_xseq, 0, 8));
+    CUDA_TRY(cudaMalloc((void**)&h->d_xseq, 4));
+    CUDA_TRY(cudaMemset(h->d_xseq, 0, 4));
     CUDA_TRY(cudaDeviceSynchronize());
   }
   cudaIpcMemHandle_t hd;

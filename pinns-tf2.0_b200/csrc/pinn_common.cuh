@@ -118,12 +118,6 @@ __device__ __forceinline__ double tanh_fast(double x) {
   return copysign(qd, x);
 }
 
-// ---- programmatic dependent launch (PDL): a kernel launched with cudaLaunchAttributeProgrammaticStreamSerialization may
-// be scheduled while its predecessor in the stream still runs; pdl_wait() blocks until that predecessor has COMPLETED and
-// its memory is visible; pdl_launch_dependents() lets the successor's blocks be placed early (they park in pdl_wait).
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-
 __device__ __forceinline__ double shfl_xor_d(double v, int m) { return __shfl_xor_sync(0xffffffffu, v, m); }
 __device__ __forceinline__ double warp_sum(double v) {
 #pragma unroll

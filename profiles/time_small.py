@@ -1,5 +1,5 @@
 """Adam-step time of the small BASELINE configurations (cfg1: N_f=10000 inference; cfg4: N=2000 identification).  Run from the repo
-root; PINN_PDL=1 switches programmatic dependent launch of the tail kernel on."""
+root."""
 import os, sys, json
 import numpy as np
 sys.path.insert(0, os.getcwd())

@@ -1,7 +1,7 @@
 """Multi-GPU parity check (run under torchrun on N GPUs; driven by tests/test_gpu_multi.py and by hand):
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 --master-port 29511 tests/mgpu_check.py
 Sharded loss/gradient/Adam/L-BFGS must match the single-GPU evaluation of the whole set -- through the fused NVLink push
-exchange (reduce_exchange) AND through the NCCL path, for the Burgers and the Schrodinger kernels."""
+exchange (exchange_block) AND through the NCCL path, for the Burgers and the Schrodinger kernels."""
 import os
 import sys
 

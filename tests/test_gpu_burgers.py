@@ -383,7 +383,7 @@ print(json.dumps(out))
 
 def test_two_handles_stepping_concurrently_on_one_device():
     """Two handles enqueue asynchronous Adam steps alternately on their own streams.  Only one of two concurrent launches may keep
-    its last CTAs spinning for the in-kernel tail (pinn_api.cu: tail_slot_free); the other falls back to the tail kernels.  The run
+    its last CTAs spinning for the in-kernel tail (pinn_api.cu: tail_slot_free); the other falls back to the tail kernel.  The run
     must finish (a subprocess with a timeout guards the test session) and both trajectories must equal a handle stepped alone."""
     import json
     import os

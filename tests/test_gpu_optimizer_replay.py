@@ -189,7 +189,7 @@ ADAM_CASES = [
     ("ide_disc", "ide_disc", REF_HP, SCRIPT),
     ("ide_disc_eps", "ide_disc", EPS_HP, [("steps", 25)]),
 ]
-# Burgers runs through three different reductions + Adam: the v2 kernel's in-kernel tail, reduce_adam after v2, and v1
+# Burgers runs through three different reductions + Adam: the v2 kernel's in-kernel tail, reduce_tail after v2, and v1
 ADAM_PATHS = {"v2_tail": {"PINN_BURGERS_KERNEL": "v2"}, "v2_no_tail": {"PINN_BURGERS_KERNEL": "v2", "PINN_FUSED_TAIL": "0"},
               "v1": {"PINN_BURGERS_KERNEL": "v1"}}
 RING_STEPS = 4096 + 104
@@ -244,7 +244,7 @@ def test_adam_step_by_step_against_longdouble(adam_runs, path, case):
     if case.endswith("_eps"):
         assert run[case]["eps_dominated"]            # the case exercises what it is meant to
     # the path ran as named: one launch per step when the v2 kernel reduces and applies Adam in its own last CTAs, two (fused
-    # kernel + reduce_adam) with PINN_FUSED_TAIL=0, with v1 and with every other kernel
+    # kernel + reduce_tail) with PINN_FUSED_TAIL=0, with v1 and with every other kernel
     model = {c[0]: c[1] for c in ADAM_CASES}[case]
     assert run[case]["launches_per_step"] == [1 if path == "v2_tail" and model in ("burgers", "ide") else 2], run[case]
 

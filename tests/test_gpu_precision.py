@@ -433,55 +433,3 @@ def test_lbfgs_at_the_instantiation_switch_points(cabi, layers):
     assert r["n_iter"] == tr.n_iter == 5 and r["n_eval"] == tr.n_eval
     rel = lambda a, b: np.linalg.norm(np.asarray(a) - np.asarray(b)) / np.linalg.norm(np.asarray(b))
     assert rel(r["f_hist"], tr.f_hist) < 1e-7 and rel(r["x_final"], tr.x_final) < 1e-7
-
-
-# --------------------------------------------------------------------------------------- programmatic dependent launch (PDL)
-PDL_STEPS, PDL_LR = 25, 0.01
-PDL_GENERIC = [2, 24, 12, 24, 1]
-
-
-def _pdl_problems():
-    gn, gb = load_golden("nls_inf"), load_golden("burgers_inf")
-    return gn, gb, _rand_w(PDL_GENERIC, 5)
-
-
-def pdl_worker():
-    c = _cabi()
-    gn, gb, wg = _pdl_problems()
-    out = {}
-    p = c.Pinn(c.NLS_INF, NLS, gn["lb"], gn["ub"])
-    p.set_collocation(gn["X_f"][:, 0], gn["X_f"][:, 1]); p.set_boundary(gn["tb"]); p.set_data(gn["x0"], gn["uv0"])
-    p.set_weights(gn["w"])
-    q = c.Pinn(c.BURGERS_INF, PDL_GENERIC, gb["lb"], gb["ub"])
-    q.set_pde_params([float(gb["nu"])]); q.set_collocation(gb["X_f"][:, 0], gb["X_f"][:, 1]); q.set_data(gb["X_u"], gb["u"])
-    q.set_weights(wg)
-    for _ in range(PDL_STEPS):
-        p.adam_step(PDL_LR, sync=False)
-        q.adam_step(PDL_LR, sync=False)
-    for name, h in (("nls", p), ("generic", q)):
-        h.sync()
-        out[name] = {"w": h.get_weights().tolist(), "loss": h.last_loss()}
-        h.close()
-    print(json.dumps(out))
-
-
-def test_programmatic_dependent_launch_leaves_the_trajectory_unchanged():
-    """PINN_PDL=1 lets the tail kernels (reduction + Adam) be placed while the fused kernel drains; the summation order is the
-    same, so 25 asynchronous Adam steps must give the same bits as without it, and the oracle's Adam trajectory."""
-    res = {flag: run_worker("pdl_worker", {"PINN_PDL": flag}) for flag in ("0", "1")}
-    for name in ("nls", "generic"):
-        assert res["1"][name]["w"] == res["0"][name]["w"] and res["1"][name]["loss"] == res["0"][name]["loss"], name
-    gn, gb, wg = _pdl_problems()
-    ops = {
-        "nls": (gn["w"], lambda x: ty.schrodinger_loss_grad(x, NLS, gn["lb"], gn["ub"], gn["X_f"], gn["tb"], gn["x0"], gn["uv0"])),
-        "generic": (wg, lambda x: ty.burgers_loss_grad(x, PDL_GENERIC, gb["lb"], gb["ub"], gb["X_f"], gb["X_u"], gb["u"],
-                                                       nu=float(gb["nu"]))),
-    }
-    for name, (w, op) in ops.items():
-        st = rp.adam_init(w.size)
-        for _ in range(PDL_STEPS):
-            f, g = op(w)[:2]
-            w = rp.adam_update(w, g, st, PDL_LR)
-        got = np.array(res["1"][name]["w"])
-        assert np.linalg.norm(got - w) / np.linalg.norm(w) < 1e-8, name
-        assert abs(res["1"][name]["loss"] - f) <= 1e-8 * abs(f), name
