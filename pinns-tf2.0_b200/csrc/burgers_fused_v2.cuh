@@ -50,6 +50,11 @@
 // weight-gradient DMMAs with __nanosleep between k-steps, and a THREE-warps-per-sub-partition variant that splits every tile's
 // chain between two half-warps (N tiles {0,2} / {1}, A operands from shared memory, roles alternating per layer; 384 threads x
 // 168 registers: pair barriers and the A-operand LDS cost more than the added latency hiding bought).
+// Tried on the H100 and dropped as slower (DESIGN §6): each layer's elementwise work fused slot by slot with the GEMM that
+// consumes it (k-step j right after slot j; staging, ring arrive and the next layer's loads after the DMMA issue;
+// profiles/experiments/burgers_chain_slotwise.patch).  Bit-identical, 51 instead of 13 DMMA.16x8x4 next to FP64 arithmetic in
+// the SASS, and 0.5 % slower: DMMA.16x8 interleaved with DFMA in one warp costs more than the latency it hides.  Fully
+// unrolled layer loops (no spills; 9-11 k instead of 7 k SASS instructions): forward +5 %, backward +1 %, both +18 %.
 #pragma once
 #include "burgers_fused.cuh"
 
@@ -525,11 +530,11 @@ __global__ void __maxnreg__(252) fused_loss_grad(const Args p) {
         }
       }
       pc.mark(PH_OUT);
-      // ---------------- backward: layers 7..1 (task J = 7-l, ring slot J % RING)
+      // ---------------- backward: layers 7..1 (task J = 7-l, ring slot J % RING); V holds the outputs of layer l (l = 7: still in
+      // registers from the forward pass)
 #pragma unroll 1
       for (int l = NHID - 1; l >= 1; l--) {
         const int T = 7 * it + (7 - l), slot = T % RING;
-        if (l < NHID - 1) load5(V, stash + STASH0 + (l - 1) * STASHL, lane);        // outputs of layer l (l = 7: registers)
         act_backward5(A, V);                                                         // A := Z-bar
         pc.mark(PH_BWD_ACT);
         if (T >= RING) wait_consumed(bars, c, T - RING);                             // the slot's previous task is done
@@ -547,6 +552,9 @@ __global__ void __maxnreg__(252) fused_loss_grad(const Args p) {
 #pragma unroll
             for (int nt = 0; nt < 3; nt++) An[s][nt][0] = An[s][nt][1] = 0.0;
           if (!PINN_ABL_NODMMA) mma_layer5(An, A, Wl, 1, W, lane);
+          // the outputs of layer l-1 (STASH0 == STASHL), loaded while the DMMAs are in flight: issued before the GEMM's
+          // results are needed, their shared-memory latency is hidden instead of starting the next layer's arithmetic
+          load5(V, stash + (l - 1) * STASHL, lane);
           c_to_v5(A, An, lane);
         }
         pc.mark(PH_BWD_GEMM);
@@ -554,7 +562,6 @@ __global__ void __maxnreg__(252) fused_loss_grad(const Args p) {
       // ---------------- backward: layer 0: its weight gradient is 3 rows (x^, t^, bias) -- 25 FMAs per lane here instead of 24
       // DMMAs in a weight-gradient warp
       {
-        load5(V, stash, lane);
         act_backward5(A, V);
 #pragma unroll
         for (int j = 0; j < 5; j++) {
