@@ -40,7 +40,12 @@ enum {
                            net [1, ..., q+1] on x only; U_0 = U_1 + dt (U U_x - nu U_xx) IRK^T; SSE losses          */
   PINN_BURGERS_IDE_DISC = 4 /* 1d-burgers/ide_disc_burgers.py:48-203  discrete-time identification: net [1, ..., q], two
                            snapshots; N = l1 U U_x - exp(l2) U_xx; U_0 = U + dt N alpha^T, U_1 = U - dt N (beta-alpha)^T;
-                           loss = sum (U_0 - u_0)^2 + sum (U_1 - u_1)^2; flat vector ends with [lambda_1, lambda_2]   */
+                           loss = sum (U_0 - u_0)^2 + sum (U_1 - u_1)^2; flat vector ends with [lambda_1, lambda_2]   */,
+  PINN_KDV_IDE_DISC = 5, /* discrete_time_identification (KdV)/KdV.py of PINNs/main (fp64 restatement): as BURGERS_IDE_DISC
+                           with u_t + l1 u u_x + exp(l2) u_xxx = 0, i.e. N = l1 U U_x + exp(l2) U_xxx; net [1, ..., q]    */
+  PINN_AC_DISC = 6      /* discrete_time_inference (AC)/AC.py of PINNs/main (fp64 restatement): net [1, ..., q+1] on x;
+                           N = k U^3 - k U - d U_xx; U_0 = U_1 + dt N IRK^T; loss = sum (U_0 - u_0)^2 + sum over all q+1
+                           outputs of (U_1(lb) - U_1(ub))^2 + (d/dx U_1(lb) - d/dx U_1(ub))^2 (periodic in value and slope) */
 };
 
 /* L-BFGS stop reasons (utils/custom_lbfgs.py:73-76,154-156,192-215). */
@@ -81,17 +86,19 @@ int pinn_p2p_enable(pinn_t* h, int on);
 int64_t pinn_num_params(const pinn_t* h);
 
 /* PDE constants.  BURGERS_INF: p[0] = nu (inf_cont_burgers.py:52,111).  BURGERS_DISC: p = [nu, dt]
- * (inf_disc_burgers.py:53-54).  BURGERS_IDE_DISC: p = [dt] (ide_disc_burgers.py:52).  Others take none. */
+ * (inf_disc_burgers.py:53-54).  BURGERS_IDE_DISC and KDV_IDE_DISC: p = [dt] (ide_disc_burgers.py:52).
+ * AC_DISC: p = [dt, d, k].  Others take none. */
 int pinn_set_pde_params(pinn_t* h, const double* p, int n);
 /* get_params(numpy=True): BURGERS_INF -> [nu] (inf_cont_burgers.py:92-93); BURGERS_IDE and BURGERS_IDE_DISC ->
  * [lambda_1, exp(lambda_2)] read from the trained flat vector (ide_cont_burgers.py:109-114, ide_disc_burgers.py:138-143);
- * BURGERS_DISC -> [nu, dt]. */
+ * KDV_IDE_DISC -> [lambda_1, exp(lambda_2)] likewise; BURGERS_DISC -> [nu, dt]; AC_DISC -> [dt, d, k]. */
 int pinn_get_params(pinn_t* h, double* p, int n);
 /* BURGERS_DISC: the implicit Runge-Kutta stage matrix IRK_weights, (q+1) x q row-major (inf_disc_burgers.py:56,86);
  * q+1 must equal the network's output width.
  * BURGERS_IDE_DISC: irk = [M_0 ; M_1], 2q x q row-major, with M_0 = IRK_alpha and M_1 = -(IRK_beta - IRK_alpha) (the caller
  * forms the difference exactly as the reference does -- in the tables' float32, ide_disc_burgers.py:107 -- and folds the sign
  * of N' = -N into it); q must equal the network's output width. */
+/* KDV_IDE_DISC takes the BURGERS_IDE_DISC layout, AC_DISC the BURGERS_DISC one. */
 int pinn_set_irk(pinn_t* h, const double* irk, int q);
 
 /* Collocation points of THIS rank: x_f, t_f (inf_cont_burgers.py:55-56; inf_cont_schrodinger.py:56-57).
@@ -106,10 +113,11 @@ int pinn_set_collocation_mapped(pinn_t* h, const double* x_pinned, const double*
 /* Data term: X_u,u of fit(X_u,u) (utils/neuralnetwork.py:138-146).  X is (n,in_dim) row-major; in_dim==1
  * reproduces the Lambda's broadcast of a (N,1) input to (x, t:=x) (quirk Q1, inf_cont_schrodinger.py:164).
  * u is (n,out_dim).  For BURGERS_IDE these are also the residual points (ide_cont_burgers.py:88-91,116-118).
- * weight: 1 on the rank that owns the (replicated) data term, 0 elsewhere. */
+ * weight: 1 on the rank that owns the (replicated) data term, 0 elsewhere.
+ * AC_DISC: x_0 (n,1) and u_0 (n,1); the periodic pair is (lb[0], ub[0]) of pinn_create, so it needs no pinn_set_boundary. */
 int pinn_set_data(pinn_t* h, const double* X, int64_t n, int in_dim, const double* u, int out_dim, double weight);
 
-/* BURGERS_IDE_DISC: snapshot `which` (0: (x_0,u_0) at t_0, 1: (x_1,u_1) at t_1 = t_0 + dt) of fit(x_0,u_0,x_1,u_1)
+/* BURGERS_IDE_DISC and KDV_IDE_DISC: snapshot `which` (0: (x_0,u_0) at t_0, 1: (x_1,u_1) at t_1 = t_0 + dt) of fit(x_0,u_0,x_1,u_1)
  * (ide_disc_burgers.py:149-156); x and u are (n,1), u broadcasts over the q stages.  pinn_set_data == snapshot 0. */
 int pinn_set_snapshot(pinn_t* h, int which, const double* x, int64_t n, const double* u);
 

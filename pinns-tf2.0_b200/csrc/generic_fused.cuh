@@ -1,6 +1,7 @@
-// Generic fused PINN loss + gradient kernel: ANY tanh MLP [2, w_1, ..., w_k, out] (widths <= 128, <= 15 Dense layers),
+// Generic fused PINN loss + gradient kernel: ANY tanh MLP [2, w_1, ..., w_k, out] (hidden widths <= 256, <= 15 Dense layers),
 // PDE heads: Burgers inference / identification (out = 1), Schrodinger (out = 2), and the discrete-time (implicit
-// Runge-Kutta) Burgers model [1, ..., q+1] of 1d-burgers/inf_disc_burgers.py (1-D input, q+1 <= 512 outputs); fp64, sm_90a.
+// Runge-Kutta) models on 1-D nets [1, ..., q(+1)] (q+1 <= 512 outputs): Burgers inference and identification
+// (1d-burgers/inf_disc_burgers.py, ide_disc_burgers.py), KdV identification and Allen-Cahn inference; fp64, sm_90a.
 //
 // Purpose: hp["layers"] is user-configurable in the reference (1d-burgers/inf_cont_burgers.py:23-34); the DMMA kernels
 // (burgers_fused_v2.cuh, nls_fused.cuh) are specialised for the two BASELINE nets.  This kernel keeps the path a drop-in
@@ -15,6 +16,8 @@
 //   HEAD  linear head, PDE residual / data / boundary terms, loss parts, seeds
 //   B_l   Z-bar (division-free backward formula) -> weight gradient (thread per weight entry, loop over the CTA's points;
 //         written once per CTA) -> input adjoint (thread per (point, unit))
+// Third-order mode (o3, KdV): a 1-D net has no t stream, so its slot carries h_xxx instead (input h_xxx = 0).  Only the
+// tanh epilogue of the forward and the Z-bar formulas change; every contraction is the same 4-stream one.
 #pragma once
 #include "optim_kernels.cuh"
 
@@ -32,13 +35,16 @@ struct Args {
   const double* tgt;          // data targets [n_d][out]
   long long n_total;
   int pde;                    // PINN_BURGERS_INF / PINN_BURGERS_IDE / PINN_NLS_INF / PINN_BURGERS_DISC (3) / PINN_BURGERS_IDE_DISC (4)
+                              // / PINN_KDV_IDE_DISC (5) / PINN_AC_DISC (6)
   int in_dim;                 // 2 (x,t), or 1 (x only: discrete-time models)
-  double dt;                  // DISC: time step;  irk: (q+1) x q stage matrix, q = out - 1;  IDE_DISC: [M_0 ; M_1], each q x q, q = out
+  int o3;                     // third-order mode: the t slot carries the xxx stream (KdV)
+  double dt;                  // DISC, AC: time step;  irk: (q+1) x q stage matrix, q = out - 1;  IDE_DISC, KdV: [M_0 ; M_1], each q x q, q = out
+  double kc;                  // AC: k of k u^3 - k u (its d is in nu)
   const double* irk;
   // Burgers: points [d0, d0+n_d) carry the data term, [c0, c0+n_c) the residual term
   long long c0, n_c, d0, n_d;
   double wf, wd, nu;
-  // NLS: [ic n0 | pad to n0p | (lb,ub) pairs 2 nb | collocation]
+  // NLS: [ic n0 | pad to n0p | (lb,ub) pairs 2 nb | collocation];  AC: [x_0 n_d | pad to n0p | (lb, ub)]
   long long n0, n0p, nb;
   double w0, wb;
   int p_net;                  // network parameters (identification: lambdas at p_net, p_net+1)
@@ -126,6 +132,149 @@ __device__ __forceinline__ void block_reduce_store(double v, double* red, double
   }
 }
 
+// Discrete-time IRK heads (pde 3..6), out of line: this code runs once per evaluation, and inlined it would take registers
+// from the hidden-layer loops.  Returns (part0, part1, d/d lambda_1, d/d lambda_2) of this thread.
+struct HeadSums { double part0, part1, gl1, gl2; };
+struct DiscArgs { const double* irk; const double* tgt; long long n_d, n0p; double dt, nu, kc; int pde; };
+__device__ __noinline__ HeadSums disc_head(const DiscArgs p, int npts, int out, long long base, const double* OUTV, double* SEED,
+                                          double* NB, double* RB, double l1, double kap) {
+  const int tid = threadIdx.x, lane = tid & 31;
+  double part0 = 0.0, part1 = 0.0, gl1 = 0.0, gl2 = 0.0;
+  // Discrete-time IRK heads.  OUTV[pt] = [U (out) | U_x | (t: 0; KdV: U_xxx) | U_xx].
+  // pde 3, inference (1d-burgers/inf_disc_burgers.py:61-101), out = q+1:
+  //   N_j = U_j U_x,j - nu U_xx,j (j < q);  U_0,k = U_k + dt sum_j N_j IRK[k][j];  loss = sum (U_0 - u_0)^2 on the data
+  //   points + sum U^2 on the boundary points.
+  // pde 4, identification (1d-burgers/ide_disc_burgers.py:81-115), out = q, two snapshots [x_0 (n_d) | x_1]:
+  //   N_j = l1 U_j U_x,j - e^{l2} U_xx,j;  snapshot s: pred_k = U_k + dt sum_j N_j M_s[k][j] with M_0 = alpha and
+  //   M_1 = -(beta - alpha) (the sign of N' = -N folded into the matrix);  loss = sum (pred - u_s)^2 over points and stages.
+  // pde 5, KdV identification: as pde 4 with N_j = l1 U_j U_x,j + e^{l2} U_xxx,j (third-order mode).
+  // pde 6, Allen-Cahn inference: as pde 3 with N_j = k U_j^3 - k U_j - d U_xx,j; the boundary term is the periodic pair
+  //   (lb, ub) at [n0p, n0p + 2): sum_k (U_k(lb) - U_k(ub))^2 + (U_x,k(lb) - U_x,k(ub))^2 over all q+1 outputs.
+  // Scratch: NB[pt][q] (N, then N-bar), RB[pt][out] (2 x residual).
+  const bool kdv = p.pde == 5, ac = p.pde == 6;
+  const bool idd = p.pde == 4 || kdv;
+  const int q = idd ? out : out - 1;
+  for (int idx = tid; idx < npts * q; idx += THREADS) {
+    const int pt = idx / q, j = idx - pt * q;
+    const double* o = OUTV + (size_t)pt * 4 * out;
+    if (kdv) NB[idx] = fma(l1 * o[j], o[out + j], kap * o[2 * out + j]);
+    else if (ac) NB[idx] = fma(p.kc * o[j], o[j] * o[j], -p.kc * o[j]) - p.nu * o[3 * out + j];
+    else NB[idx] = l1 * o[j] * o[out + j] - kap * o[3 * out + j];       // inference: l1 = 1, kap = nu
+  }
+  __syncthreads();
+  // (i) stage products  S[pt][k] = sum_j N[pt][j] M_pt[k][j]  -> RB.  One warp per (point, stage), lanes over j: the rows of the
+  // stage matrix are read coalesced and all 16 loads of a lane are in flight at once (q <= 512).  (Round 1: a thread per
+  // (point, stage) walking its own row -- 41 % of this model's step.)
+  for (int it = tid >> 5; it < npts * out; it += THREADS / 32) {
+    const int pt = it / out, k = it - pt * out;
+    const long long gp = base + pt;
+    if (idd || gp < p.n_d) {
+      const double* nrow = NB + (size_t)pt * q;
+      const double* irow = p.irk + ((idd && gp >= p.n_d) ? (size_t)q * q : 0) + (size_t)k * q;
+      double mv[16], nv[16];
+#pragma unroll
+      for (int c = 0; c < 16; c++) {
+        const int j = lane + 32 * c;
+        mv[c] = j < q ? __ldg(irow + j) : 0.0;
+        nv[c] = j < q ? nrow[j] : 0.0;
+      }
+      double acc = 0.0;
+#pragma unroll
+      for (int c = 0; c < 16; c++) acc = fma(nv[c], mv[c], acc);
+      acc = warp_sum(acc);
+      if (lane == 0) RB[it] = acc;
+    }
+  }
+  __syncthreads();
+  for (int idx = tid; idx < npts * out; idx += THREADS) {
+    const int pt = idx / out, k = idx - pt * out;
+    const long long gp = base + pt;
+    const double uk = OUTV[(size_t)pt * 4 * out + k];
+    if (idd || gp < p.n_d) {
+      const bool second = idd && gp >= p.n_d;
+      const double r = fma(p.dt, RB[idx], uk) - __ldg(p.tgt + gp);  // targets: [u_0 | u_1]
+      if (second) part1 = fma(r, r, part1); else part0 = fma(r, r, part0);
+      RB[idx] = 2.0 * r;
+    } else if (ac) {
+      // periodic pair: lb at an even offset from n0p, its ub partner next to it in the same CTA (pts and n0p are even)
+      double dv = 0.0;
+      if (gp >= p.n0p) {
+        const bool is_lb = ((gp - p.n0p) & 1) == 0;
+        const double* o = OUTV + (size_t)pt * 4 * out;
+        const double* op = o + (is_lb ? 4 * out : -4 * out);
+        dv = o[k] - op[k];
+        const double dx = o[out + k] - op[out + k];
+        if (is_lb) part1 = fma(dv, dv, fma(dx, dx, part1));
+      }
+      RB[idx] = 2.0 * dv;                  // 0 on the alignment pad
+    } else {
+      part1 = fma(uk, uk, part1);
+      RB[idx] = 2.0 * uk;                  // boundary point: d/dU of sum U^2
+    }
+  }
+  __syncthreads();
+  // (ii) N-bar[pt][j] = dt sum_k RB[pt][k] M_pt[k][j]: thread per (point, column j) (coalesced over j), the k loop unrolled so
+  // that 16 independent matrix loads are in flight per thread
+  for (int idx = tid; idx < npts * q; idx += THREADS) {
+    const int pt = idx / q, j = idx - pt * q;
+    const long long gp = base + pt;
+    double acc = 0.0;
+    if (idd || gp < p.n_d) {
+      const double* rrow = RB + (size_t)pt * out;
+      const double* mcol = p.irk + ((idd && gp >= p.n_d) ? (size_t)q * q : 0) + j;
+      double a0 = 0.0, a1 = 0.0, a2 = 0.0, a3 = 0.0;
+      int k = 0;
+      for (; k + 16 <= out; k += 16) {
+        double mv[16];
+#pragma unroll
+        for (int c = 0; c < 16; c++) mv[c] = __ldg(mcol + (size_t)(k + c) * q);
+#pragma unroll
+        for (int c = 0; c < 16; c += 4) {
+          a0 = fma(rrow[k + c], mv[c], a0);
+          a1 = fma(rrow[k + c + 1], mv[c + 1], a1);
+          a2 = fma(rrow[k + c + 2], mv[c + 2], a2);
+          a3 = fma(rrow[k + c + 3], mv[c + 3], a3);
+        }
+      }
+      for (; k < out; k++) a0 = fma(rrow[k], __ldg(mcol + (size_t)k * q), a0);
+      acc = ((a0 + a1) + (a2 + a3)) * p.dt;
+    }
+    NB[idx] = acc;                          // N-bar (0 on boundary points)
+  }
+  __syncthreads();
+  for (int idx = tid; idx < npts * out; idx += THREADS) {
+    const int pt = idx / out, k = idx - pt * out;
+    const double* o = OUTV + (size_t)pt * 4 * out;
+    const double nb_ = k < q ? NB[(size_t)pt * q + k] : 0.0;
+    double* sdp = SEED + (size_t)pt * 4 * out;
+    if (kdv) {
+      sdp[k] = fma(nb_ * l1, o[out + k], RB[idx]);
+      sdp[out + k] = nb_ * l1 * o[k];
+      sdp[2 * out + k] = kap * nb_;
+      sdp[3 * out + k] = 0.0;
+      gl1 = fma(nb_ * o[k], o[out + k], gl1);
+      gl2 = fma(kap * nb_, o[2 * out + k], gl2);
+    } else if (ac) {
+      const long long gp = base + pt;
+      double sx = 0.0;                                               // slope seed of the periodic pair: 2 (U_x - U_x(partner))
+      if (gp >= p.n0p) sx = 2.0 * (o[out + k] - o[(((gp - p.n0p) & 1) == 0 ? 4 * out : -4 * out) + out + k]);
+      sdp[k] = fma(nb_, fma(3.0 * p.kc * o[k], o[k], -p.kc), RB[idx]);
+      sdp[out + k] = sx;
+      sdp[2 * out + k] = 0.0;
+      sdp[3 * out + k] = -p.nu * nb_;
+    } else {
+      sdp[k] = fma(nb_ * l1, o[out + k], RB[idx]);
+      sdp[out + k] = nb_ * l1 * o[k];
+      sdp[2 * out + k] = 0.0;
+      sdp[3 * out + k] = -kap * nb_;
+      gl1 = fma(nb_ * o[k], o[out + k], gl1);                       // d/d lambda_1, d/d lambda_2 (raw); unused for pde 3
+      gl2 = fma(-kap * nb_, o[3 * out + k], gl2);
+    }
+  }
+  __syncthreads();
+  return {part0, part1, gl1, gl2};
+}
+
 __global__ void __launch_bounds__(THREADS, 2) fused_loss_grad(const Args p) {
   __shared__ double red[THREADS / 32];
   __shared__ int work_ctr;
@@ -146,7 +295,8 @@ __global__ void __launch_bounds__(THREADS, 2) fused_loss_grad(const Args p) {
   double* SEED = OUTV + (size_t)pts * 4 * out;
   double* outp = p.partials + (size_t)blockIdx.x * p.pstride;
   const double sc0 = 2.0 / nd.dx0, sc1 = 2.0 / nd.dx1;
-  const bool ide = p.pde == 1 || p.pde == 4;
+  const bool ide = p.pde == 1 || p.pde == 4 || p.pde == 5;
+  const bool o3 = p.o3 != 0;
   const double l1 = ide ? p.w[p.p_net] : 1.0;
   const double kap = ide ? exp(p.w[p.p_net + 1]) : p.nu;
 
@@ -198,7 +348,7 @@ __global__ void __launch_bounds__(THREADS, 2) fused_loss_grad(const Args p) {
                 double* o = Ho + (size_t)pt * fo + u;
                 o[0] = a;
                 o[so] = sd * zx;
-                o[2 * so] = sd * C[2][j][e];
+                o[2 * so] = sd * (o3 ? xxx_bracket(a, zx, C[3][j][e], C[2][j][e]) : C[2][j][e]);
                 o[3 * so] = sd * fma(-2.0 * a * zx, zx, C[3][j][e]);
               }
             }
@@ -230,7 +380,7 @@ __global__ void __launch_bounds__(THREADS, 2) fused_loss_grad(const Args p) {
       double* o = Ho + (size_t)pt * fo + j;
       o[0] = a;
       o[so] = s * zx;
-      o[2 * so] = s * zt;
+      o[2 * so] = s * (o3 ? xxx_bracket(a, zx, zxx, zt) : zt);
       o[3 * so] = s * fma(-2.0 * a * zx, zx, zxx);
     }
     __syncthreads();
@@ -251,105 +401,10 @@ __global__ void __launch_bounds__(THREADS, 2) fused_loss_grad(const Args p) {
   }
   __syncthreads();
   double part0 = 0.0, part1 = 0.0, part2 = 0.0, gl1 = 0.0, gl2 = 0.0;
-  if (p.pde == 3 || p.pde == 4) {
-    // Discrete-time IRK heads.  OUTV[pt] = [U (out) | U_x | (t: 0) | U_xx].
-    // pde 3, inference (1d-burgers/inf_disc_burgers.py:61-101), out = q+1:
-    //   N_j = U_j U_x,j - nu U_xx,j (j < q);  U_0,k = U_k + dt sum_j N_j IRK[k][j];  loss = sum (U_0 - u_0)^2 on the data
-    //   points + sum U^2 on the boundary points.
-    // pde 4, identification (1d-burgers/ide_disc_burgers.py:81-115), out = q, two snapshots [x_0 (n_d) | x_1]:
-    //   N_j = l1 U_j U_x,j - e^{l2} U_xx,j;  snapshot s: pred_k = U_k + dt sum_j N_j M_s[k][j] with M_0 = alpha and
-    //   M_1 = -(beta - alpha) (the sign of N' = -N folded into the matrix);  loss = sum (pred - u_s)^2 over points and stages.
-    // Scratch: NB[pt][q] (N, then N-bar), RB[pt][out] (2 x residual).
-    const bool idd = p.pde == 4;
-    const int q = idd ? out : out - 1;
-    double* NB = A0;
-    double* RB = A1;
-    for (int idx = tid; idx < npts * q; idx += THREADS) {
-      const int pt = idx / q, j = idx - pt * q;
-      const double* o = OUTV + (size_t)pt * 4 * out;
-      NB[idx] = l1 * o[j] * o[out + j] - kap * o[3 * out + j];       // inference: l1 = 1, kap = nu
-    }
-    __syncthreads();
-    // (i) stage products  S[pt][k] = sum_j N[pt][j] M_pt[k][j]  -> RB.  One warp per (point, stage), lanes over j: the rows of the
-    // stage matrix are read coalesced and all 16 loads of a lane are in flight at once (q <= 512).  (Round 1: a thread per
-    // (point, stage) walking its own row -- 41 % of this model's step.)
-    for (int it = tid >> 5; it < npts * out; it += THREADS / 32) {
-      const int pt = it / out, k = it - pt * out;
-      const long long gp = base + pt;
-      if (idd || gp < p.n_d) {
-        const double* nrow = NB + (size_t)pt * q;
-        const double* irow = p.irk + ((idd && gp >= p.n_d) ? (size_t)q * q : 0) + (size_t)k * q;
-        double mv[16], nv[16];
-#pragma unroll
-        for (int c = 0; c < 16; c++) {
-          const int j = lane + 32 * c;
-          mv[c] = j < q ? __ldg(irow + j) : 0.0;
-          nv[c] = j < q ? nrow[j] : 0.0;
-        }
-        double acc = 0.0;
-#pragma unroll
-        for (int c = 0; c < 16; c++) acc = fma(nv[c], mv[c], acc);
-        acc = warp_sum(acc);
-        if (lane == 0) RB[it] = acc;
-      }
-    }
-    __syncthreads();
-    for (int idx = tid; idx < npts * out; idx += THREADS) {
-      const int pt = idx / out, k = idx - pt * out;
-      const long long gp = base + pt;
-      const double uk = OUTV[(size_t)pt * 4 * out + k];
-      if (idd || gp < p.n_d) {
-        const bool second = idd && gp >= p.n_d;
-        const double r = fma(p.dt, RB[idx], uk) - __ldg(p.tgt + gp);  // targets: [u_0 | u_1]
-        if (second) part1 = fma(r, r, part1); else part0 = fma(r, r, part0);
-        RB[idx] = 2.0 * r;
-      } else {
-        part1 = fma(uk, uk, part1);
-        RB[idx] = 2.0 * uk;                  // boundary point: d/dU of sum U^2
-      }
-    }
-    __syncthreads();
-    // (ii) N-bar[pt][j] = dt sum_k RB[pt][k] M_pt[k][j]: thread per (point, column j) (coalesced over j), the k loop unrolled so
-    // that 16 independent matrix loads are in flight per thread
-    for (int idx = tid; idx < npts * q; idx += THREADS) {
-      const int pt = idx / q, j = idx - pt * q;
-      const long long gp = base + pt;
-      double acc = 0.0;
-      if (idd || gp < p.n_d) {
-        const double* rrow = RB + (size_t)pt * out;
-        const double* mcol = p.irk + ((idd && gp >= p.n_d) ? (size_t)q * q : 0) + j;
-        double a0 = 0.0, a1 = 0.0, a2 = 0.0, a3 = 0.0;
-        int k = 0;
-        for (; k + 16 <= out; k += 16) {
-          double mv[16];
-#pragma unroll
-          for (int c = 0; c < 16; c++) mv[c] = __ldg(mcol + (size_t)(k + c) * q);
-#pragma unroll
-          for (int c = 0; c < 16; c += 4) {
-            a0 = fma(rrow[k + c], mv[c], a0);
-            a1 = fma(rrow[k + c + 1], mv[c + 1], a1);
-            a2 = fma(rrow[k + c + 2], mv[c + 2], a2);
-            a3 = fma(rrow[k + c + 3], mv[c + 3], a3);
-          }
-        }
-        for (; k < out; k++) a0 = fma(rrow[k], __ldg(mcol + (size_t)k * q), a0);
-        acc = ((a0 + a1) + (a2 + a3)) * p.dt;
-      }
-      NB[idx] = acc;                          // N-bar (0 on boundary points)
-    }
-    __syncthreads();
-    for (int idx = tid; idx < npts * out; idx += THREADS) {
-      const int pt = idx / out, k = idx - pt * out;
-      const double* o = OUTV + (size_t)pt * 4 * out;
-      const double nb_ = k < q ? NB[(size_t)pt * q + k] : 0.0;
-      double* sdp = SEED + (size_t)pt * 4 * out;
-      sdp[k] = fma(nb_ * l1, o[out + k], RB[idx]);
-      sdp[out + k] = nb_ * l1 * o[k];
-      sdp[2 * out + k] = 0.0;
-      sdp[3 * out + k] = -kap * nb_;
-      gl1 = fma(nb_ * o[k], o[out + k], gl1);                         // d/d lambda_1, d/d lambda_2 (raw); unused for pde 3
-      gl2 = fma(-kap * nb_, o[3 * out + k], gl2);
-    }
+  if (p.pde >= 3) {
+    const DiscArgs da{p.irk, p.tgt, p.n_d, p.n0p, p.dt, p.nu, p.kc, p.pde};
+    const HeadSums hs = disc_head(da, npts, out, base, OUTV, SEED, A0, A1, l1, kap);
+    part0 = hs.part0; part1 = hs.part1; gl1 = hs.gl1; gl2 = hs.gl2;
     __syncthreads();
   } else
   for (int pt = tid; pt < npts; pt += THREADS) {
@@ -486,6 +541,24 @@ __global__ void __launch_bounds__(THREADS, 2) fused_loss_grad(const Args p) {
       for (size_t o = 0; o < bytes; o += 65536) prefetch_l2_bulk(reinterpret_cast<const char*>(Hp) + o, (uint32_t)min((size_t)65536, bytes - o));
     }
     // (1) Z-bar
+    if (p.o3) {
+      // third-order mode (t slot = xxx stream: at = a_xxx, Bt its adjoint), in layer outputs the t-stream formula plus
+      //   Z += -6 a_x a_xx Bt,  Z_x += -6 u2 Bt,  Z_xx += -6 a a_x Bt;  Z_xxx = s Bt
+      for (int idx = tid; idx < npts * fo; idx += THREADS) {
+        const size_t q = idx;
+        const double a = Ho[q], ax = Ho[so + q], at = Ho[2 * so + q], axx = Ho[3 * so + q];
+        const double B0 = Acur[q], Bx = Acur[so + q], Bt = Acur[2 * so + q], Bxx = Acur[3 * so + q];
+        const double s = fma(-a, a, 1.0);
+        const double u1 = fma(ax, Bx, at * Bt);
+        const double u2 = fma(a, axx, ax * ax);
+        double z = fma(-2.0 * a, u1, s * B0);
+        z = fma(-2.0 * Bxx, u2, z);
+        Aoth[q] = fma(-6.0 * ax * axx, Bt, z);
+        Aoth[so + q] = fma(-6.0 * u2, Bt, fma(-4.0 * a * ax, Bxx, s * Bx));
+        Aoth[2 * so + q] = s * Bt;
+        Aoth[3 * so + q] = fma(-6.0 * a * ax, Bt, s * Bxx);
+      }
+    } else
     for (int idx = tid; idx < npts * fo; idx += THREADS) {
       const size_t q = idx;                               // == pt*fo + j
       const double a = Ho[q], ax = Ho[so + q], at = Ho[2 * so + q], axx = Ho[3 * so + q];

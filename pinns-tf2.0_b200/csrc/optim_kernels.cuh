@@ -797,12 +797,19 @@ lbfgs_apply(LbfgsState* __restrict__ st, double* __restrict__ w, const double* _
 }
 
 // ------------------------------------------------------------------------------------------------
-// Generic (any layer sizes, width <= MAXW) thread-per-point kernels, off the per-step path:
+// Generic (any layer sizes, hidden width <= MAXW_WIDE) thread-per-point kernels, off the per-step path:
 // forward (predict, utils/neuralnetwork.py:151-153) and forward Taylor-mode derivatives (parity probes,
 // f_model on the stored points).  Weights are read through the read-only path (warp-uniform addresses).
 // ------------------------------------------------------------------------------------------------
-constexpr int MAXW = 128;
+constexpr int MAXW = 128;        // per-thread activation arrays of mlp_forward_generic for the nets that fit
+constexpr int MAXW_WIDE = 256;   // widest hidden layer of any generic net (second instantiation above MAXW)
 constexpr int MAXL = 16;
+
+// Third-order mode of 1-D nets (the idle t slot carries the xxx stream):
+//   a_xxx = s (z_xxx - 6 a z_x z_xx - 2 (1 - 3a^2) z_x^3);  this returns the bracket.
+__device__ __forceinline__ double xxx_bracket(double a, double zx, double zxx, double zxxx) {
+  return fma(-6.0 * a * zx, zxx, fma(-2.0 * fma(-3.0 * a, a, 1.0) * zx * zx, zx, zxxx));
+}
 
 struct NetDesc {
   int n_layers;            // number of Dense layers
@@ -811,14 +818,15 @@ struct NetDesc {
   double lb0, lb1, dx0, dx1;
 };
 
-// NS = 1: values only; NS = 4: (h, h_x, h_t, h_xx)
-template <int NS>
+// NS = 1: values only; NS = 4: (h, h_x, h_t, h_xx), or (h, h_x, h_xxx, h_xx) with o3 (1-D nets).  W: widest hidden layer.
+template <int NS, int W>
 __global__ void mlp_forward_generic(const double* __restrict__ w, NetDesc nd, const double* __restrict__ X,
-                                    const double* __restrict__ Tsoa, long long n, int in_dim, double* __restrict__ out) {
+                                    const double* __restrict__ Tsoa, long long n, int in_dim, double* __restrict__ out,
+                                    int o3) {
   // points either interleaved X[n][in_dim] (Tsoa == nullptr) or SoA (X = x[n], Tsoa = t[n])
   const long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= n) return;
-  double h[NS][MAXW], z[NS][MAXW];
+  double h[NS][W], z[NS][W];
   const double x = Tsoa ? X[p] : X[p * in_dim];
   const double t = Tsoa ? Tsoa[p] : (in_dim == 1 ? x : X[p * in_dim + 1]);
   h[0][0] = 2.0 * (x - nd.lb0) / nd.dx0 - 1.0;
@@ -874,7 +882,7 @@ __global__ void mlp_forward_generic(const double* __restrict__ w, NetDesc nd, co
           const double sd = fma(-a, a, 1.0);
           const double zx = z[1][j];
           h[1][j] = sd * zx;
-          h[2][j] = sd * z[2][j];
+          h[2][j] = sd * (o3 ? xxx_bracket(a, zx, z[3][j], z[2][j]) : z[2][j]);
           h[3][j] = sd * fma(-2.0 * a * zx, zx, z[3][j]);
         }
       }

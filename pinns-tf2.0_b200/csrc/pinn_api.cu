@@ -81,10 +81,11 @@ struct pinn_handle {
   std::vector<int> layers;
   double lb[2] = {0, 0}, ub[2] = {1, 1};
   int P_net = 0, P = 0;             // net parameters; P = P_net (+2 identification)
-  double nu = 0.0, dt = 0.0;
+  double nu = 0.0, dt = 0.0;        // AC_DISC: nu holds d
+  double kc = 0.0;                  // AC_DISC: k
   double* d_irk = nullptr;          // DISC: (q+1) x q stage matrix
   int irk_q = 0;
-  std::vector<double> h_x0;         // DISC: data x positions (host copy for re-assembly); IDE_DISC: snapshot 0 (x_1 lives in h_tb)
+  std::vector<double> h_x0;         // DISC, AC: data x positions (host copy for re-assembly); IDE_DISC, KdV: snapshot 0 (x_1 lives in h_tb)
   std::vector<double> h_u0, h_u1;   // IDE_DISC: targets of the two snapshots
   cudaStream_t stream = nullptr;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
@@ -153,6 +154,10 @@ struct pinn_handle {
 };
 
 namespace {
+
+// 1-D (x only) discrete-time models; identification: two snapshots, q outputs; inference: q+1 outputs
+bool is_disc(int pde) { return pde == PINN_BURGERS_DISC || pde == PINN_BURGERS_IDE_DISC || pde == PINN_KDV_IDE_DISC || pde == PINN_AC_DISC; }
+bool is_ide_disc(int pde) { return pde == PINN_BURGERS_IDE_DISC || pde == PINN_KDV_IDE_DISC; }
 
 bool is_burgers_net(const std::vector<int>& L) {
   if (L.size() != 10 || L[0] != 2 || L[9] != 1) return false;
@@ -420,13 +425,20 @@ int launch_eval(pinn_t* h, const int* run_flag, bool fused_only = false, const A
   return launch_tail(h, run_flag, ad);
 }
 
-// DISC: data region = [x_0 data points | x_1 boundary points], right-aligned like every data block (t is unused)
+// DISC: data region = [x_0 data points | x_1 boundary points], right-aligned like every data block (t is unused).
+// AC: [x_0 | pad to even | lb, ub]: the periodic pair starts at an even index, so it never straddles a CTA.
 int disc_upload_points(pinn_t* h) {
-  const long long n_aux = h->n_d + h->n_b;
+  const bool ac = h->pde == PINN_AC_DISC;
+  const long long n0p = ac ? (h->n_d + 1) & ~1LL : h->n_d;
+  const long long n_aux = ac ? (h->n_d > 0 ? n0p + 2 : 0) : h->n_d + h->n_b;
   if (ensure_points(h, n_aux > h->n_aux ? n_aux : h->n_aux, 0)) return -1;
   h->stage_x.assign(n_aux, 0.0); h->stage_t.assign(n_aux, 0.0);
   for (long long i = 0; i < h->n_d; i++) h->stage_x[i] = h->h_x0[i];
-  for (long long i = 0; i < h->n_b; i++) h->stage_x[h->n_d + i] = h->h_tb[i];
+  if (ac && n_aux) {
+    for (long long i = h->n_d; i < n0p; i++) h->stage_x[i] = h->lb[0];    // inert alignment point
+    h->stage_x[n0p] = h->lb[0]; h->stage_x[n0p + 1] = h->ub[0];
+  }
+  for (long long i = 0; !ac && i < h->n_b; i++) h->stage_x[h->n_d + i] = h->h_tb[i];
   if (n_aux) {
     CUDA_TRY(cudaMemcpyAsync(h->d_x + h->dcap - n_aux, h->stage_x.data(), n_aux * 8, cudaMemcpyHostToDevice, h->stream));
     CUDA_TRY(cudaMemcpyAsync(h->d_t + h->dcap - n_aux, h->stage_t.data(), n_aux * 8, cudaMemcpyHostToDevice, h->stream));
@@ -438,8 +450,8 @@ int disc_upload_points(pinn_t* h) {
 
 int generic_launch_eval(pinn_t* h, const int* run_flag) {
   namespace G = pinn::generic;
-  const bool idd = h->pde == PINN_BURGERS_IDE_DISC;
-  const bool disc = h->pde == PINN_BURGERS_DISC || idd;
+  const bool idd = is_ide_disc(h->pde);
+  const bool disc = is_disc(h->pde);
   if (disc && (!h->d_irk || h->irk_q + (idd ? 0 : 1) != h->layers.back())) return fail("discrete-time model: call pinn_set_irk first");
   const bool nls = h->pde == PINN_NLS_INF, ide = h->pde == PINN_BURGERS_IDE;
   const long long n_total = disc ? h->n_aux : (nls ? h->n_aux + h->n_c : (ide ? h->n_d : h->n_d + h->n_c));
@@ -472,6 +484,7 @@ int generic_launch_eval(pinn_t* h, const int* run_flag) {
   a.x = h->d_x + (h->dcap - n_front); a.t = h->d_t + (h->dcap - n_front); a.tgt = h->d_u;
   a.n_total = n_total; a.pde = h->pde;
   a.in_dim = disc ? 1 : 2; a.dt = h->dt; a.irk = h->d_irk;
+  a.o3 = h->pde == PINN_KDV_IDE_DISC ? 1 : 0; a.kc = h->kc;
   a.c0 = ide ? 0 : h->n_d; a.n_c = ide ? h->n_d : h->n_c; a.d0 = 0; a.n_d = h->n_d;
   const long long nfg = ide ? h->n_d : h->n_c_global;
   a.wf = nfg > 0 ? 1.0 / (double)nfg : 0.0;
@@ -649,7 +662,7 @@ int pinn_create(pinn_t** out, int pde_id, int n_layers, const int* layers, const
                 int device, int rank, int world, const void* nccl_uid) {
   if (!out || !layers || !lb || !ub) return fail("pinn_create: null argument");
   if (n_layers < 3 || n_layers > pinn::MAXL) return fail("pinn_create: need 3..16 layer sizes");
-  if (pde_id < 0 || pde_id > 4) return fail("pinn_create: unknown pde_id");
+  if (pde_id < 0 || pde_id > 6) return fail("pinn_create: unknown pde_id");
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
     return fail("pinn_create: no CUDA device -- this library has no CPU fallback");
@@ -657,11 +670,11 @@ int pinn_create(pinn_t** out, int pde_id, int n_layers, const int* layers, const
   pinn_t* h = new pinn_t();
   h->pde = pde_id; h->device = device; h->rank = rank; h->world = world < 1 ? 1 : world;
   h->layers.assign(layers, layers + n_layers);
-  const bool disc = pde_id == PINN_BURGERS_DISC || pde_id == PINN_BURGERS_IDE_DISC;
+  const bool disc = is_disc(pde_id);
   for (int i = 0; i < n_layers; i++) {
     const int v = h->layers[i];
-    const int cap = (disc && i == n_layers - 1) ? 512 : pinn::MAXW;     // the IRK head may be q+1 = 501 wide
-    if (v < 1 || v > cap) { delete h; return fail("pinn_create: layer width out of range (1..128; IRK head <= 512)"); }
+    const int cap = (disc && i == n_layers - 1) ? 512 : pinn::MAXW_WIDE;     // the IRK head may be q+1 = 501 wide
+    if (v < 1 || v > cap) { delete h; return fail("pinn_create: layer width out of range (1..256; IRK head <= 512)"); }
   }
   if (h->layers[0] != (disc ? 1 : 2)) {
     delete h;
@@ -671,7 +684,7 @@ int pinn_create(pinn_t** out, int pde_id, int n_layers, const int* layers, const
   h->lb[1] = disc ? 0.0 : lb[1]; h->ub[1] = disc ? 1.0 : ub[1];            // the t axis does not exist for 1-D nets
   if (!(h->ub[0] > h->lb[0]) || !(h->ub[1] > h->lb[1])) { delete h; return fail("pinn_create: need ub > lb"); }
   const int want_out = pde_id == PINN_NLS_INF ? 2 : 1;
-  if (pde_id == PINN_BURGERS_IDE_DISC) {
+  if (is_ide_disc(pde_id)) {
     if (h->layers.back() < 1) { delete h; return fail("pinn_create: the discrete-time identification model needs q >= 1 outputs"); }
   } else if (disc) {
     if (h->layers.back() < 2) { delete h; return fail("pinn_create: the discrete-time model needs q+1 >= 2 outputs"); }
@@ -689,7 +702,7 @@ int pinn_create(pinn_t** out, int pde_id, int n_layers, const int* layers, const
   }
   h->P_net = 0;
   for (int l = 0; l + 1 < n_layers; l++) h->P_net += layers[l] * layers[l + 1] + layers[l + 1];
-  h->P = h->P_net + ((pde_id == PINN_BURGERS_IDE || pde_id == PINN_BURGERS_IDE_DISC) ? 2 : 0);
+  h->P = h->P_net + ((pde_id == PINN_BURGERS_IDE || is_ide_disc(pde_id)) ? 2 : 0);
 
 #define CREATE_TRY(expr)                                                                          \
   do {                                                                                            \
@@ -804,9 +817,14 @@ int pinn_set_pde_params(pinn_t* h, const double* p, int n) {
     h->nu = p[0]; h->dt = p[1];
     return 0;
   }
-  if (h->pde == PINN_BURGERS_IDE_DISC) {
-    if (n != 1 || !p) return fail("pinn_set_pde_params: BURGERS_IDE_DISC takes [dt]");
+  if (is_ide_disc(h->pde)) {
+    if (n != 1 || !p) return fail("pinn_set_pde_params: the discrete-time identification models take [dt]");
     h->dt = p[0];
+    return 0;
+  }
+  if (h->pde == PINN_AC_DISC) {
+    if (n != 3 || !p) return fail("pinn_set_pde_params: AC_DISC takes [dt, d, k]");
+    h->dt = p[0]; h->nu = p[1]; h->kc = p[2];
     return 0;
   }
   if (n != 0) return fail("pinn_set_pde_params: this PDE takes no constants");
@@ -820,7 +838,7 @@ int pinn_get_params(pinn_t* h, double* p, int n) {
     p[0] = h->nu;                                   // inf_cont_burgers.py:92-93
     return 0;
   }
-  if (h->pde == PINN_BURGERS_IDE || h->pde == PINN_BURGERS_IDE_DISC) {
+  if (h->pde == PINN_BURGERS_IDE || is_ide_disc(h->pde)) {
     if (n != 2) return fail("pinn_get_params: identification has two parameters (lambda_1, exp(lambda_2))");
     CUDA_TRY(cudaSetDevice(h->device));
     double lam[2];
@@ -834,14 +852,19 @@ int pinn_get_params(pinn_t* h, double* p, int n) {
     p[0] = h->nu; p[1] = h->dt;
     return 0;
   }
+  if (h->pde == PINN_AC_DISC) {
+    if (n != 3) return fail("pinn_get_params: AC_DISC has three constants (dt, d, k)");
+    p[0] = h->dt; p[1] = h->nu; p[2] = h->kc;
+    return 0;
+  }
   if (n != 0) return fail("pinn_get_params: this PDE has no parameters");
   return 0;
 }
 
 int pinn_set_irk(pinn_t* h, const double* irk, int q) {
   if (!h || !irk) return fail("pinn_set_irk: null argument");
-  if (h->pde != PINN_BURGERS_DISC && h->pde != PINN_BURGERS_IDE_DISC) return fail("pinn_set_irk: only the discrete-time models have stage matrices");
-  const bool idd = h->pde == PINN_BURGERS_IDE_DISC;
+  if (!is_disc(h->pde)) return fail("pinn_set_irk: only the discrete-time models have stage matrices");
+  const bool idd = is_ide_disc(h->pde);
   if (!idd && q + 1 != h->layers.back()) return fail("pinn_set_irk: q+1 must equal the network's output width");
   if (idd && q != h->layers.back()) return fail("pinn_set_irk: q must equal the network's output width");
   const size_t n_rows = idd ? (size_t)2 * q : (size_t)q + 1;      // identification: [M_0 ; M_1], each q x q
@@ -857,7 +880,7 @@ int pinn_set_irk(pinn_t* h, const double* irk, int q) {
 int pinn_set_collocation(pinn_t* h, const double* x, const double* t, int64_t n, int64_t n_global) {
   if (!h) return fail("null handle");
   if (h->pde == PINN_BURGERS_IDE) return fail("pinn_set_collocation: identification uses the data points as residual points");
-  if (h->pde == PINN_BURGERS_DISC || h->pde == PINN_BURGERS_IDE_DISC)
+  if (is_disc(h->pde))
     return fail("pinn_set_collocation: the discrete-time models have no collocation set (snapshot / boundary points only)");
   if (n < 0 || (n > 0 && (!x || !t))) return fail("pinn_set_collocation: bad arguments");
   if (n_global < n) return fail("pinn_set_collocation: n_global < n");
@@ -897,8 +920,8 @@ int pinn_set_data(pinn_t* h, const double* X, int64_t n, int in_dim, const doubl
   if (!h) return fail("null handle");
   if (n < 0 || (n > 0 && (!X || !u))) return fail("pinn_set_data: bad arguments");
   if (in_dim != 1 && in_dim != 2) return fail("pinn_set_data: in_dim must be 1 (broadcast quirk) or 2");
-  if (h->pde == PINN_BURGERS_IDE_DISC) return pinn_set_snapshot(h, 0, X, n, u);
-  if (h->pde == PINN_BURGERS_DISC) {
+  if (is_ide_disc(h->pde)) return pinn_set_snapshot(h, 0, X, n, u);
+  if (h->pde == PINN_BURGERS_DISC || h->pde == PINN_AC_DISC) {
     // x_0 (n,1) and u_0 (n,1): the snapshot the q stages are fitted to (inf_disc_burgers.py:98-101; u_0 broadcasts)
     if (in_dim != 1 || out_dim != 1) return fail("pinn_set_data: the discrete-time model takes x_0 (n,1) and u_0 (n,1)");
     CUDA_TRY(cudaSetDevice(h->device));
@@ -947,7 +970,7 @@ int pinn_set_data(pinn_t* h, const double* X, int64_t n, int in_dim, const doubl
 
 int pinn_set_snapshot(pinn_t* h, int which, const double* x, int64_t n, const double* u) {
   if (!h) return fail("null handle");
-  if (h->pde != PINN_BURGERS_IDE_DISC) return fail("pinn_set_snapshot: only the discrete-time identification model has two snapshots");
+  if (!is_ide_disc(h->pde)) return fail("pinn_set_snapshot: only the discrete-time identification models have two snapshots");
   if ((which != 0 && which != 1) || n < 0 || (n > 0 && (!x || !u))) return fail("pinn_set_snapshot: bad arguments");
   CUDA_TRY(cudaSetDevice(h->device));
   // host copies of both snapshots: the device blocks [x_0 | x_1] and [u_0 | u_1] are re-assembled whenever one changes
@@ -975,6 +998,7 @@ int pinn_set_boundary(pinn_t* h, const double* tb, int64_t n_b) {
     CUDA_TRY(cudaSetDevice(h->device));
     return disc_upload_points(h);
   }
+  if (h->pde == PINN_AC_DISC) return fail("pinn_set_boundary: the Allen-Cahn model's periodic pair is (lb, ub) of pinn_create");
   if (h->pde != PINN_NLS_INF) return fail("pinn_set_boundary: only the NLS and discrete-time inference problems have a boundary term");
   if (n_b < 0 || (n_b > 0 && !tb)) return fail("pinn_set_boundary: bad arguments");
   h->h_tb.assign(tb, tb + n_b);
@@ -1184,8 +1208,17 @@ static int forward_generic(pinn_t* h, const double* X, const double* dx, const d
   pinn::NetDesc nd = net_desc(h);
   const int threads = 64;
   const int blocks = (int)((n + threads - 1) / threads);
-  if (ns == 1) pinn::mlp_forward_generic<1><<<blocks, threads, 0, h->stream>>>(h->d_w, nd, dx, dt, n, in_dim, h->d_pout);
-  else pinn::mlp_forward_generic<4><<<blocks, threads, 0, h->stream>>>(h->d_w, nd, dx, dt, n, in_dim, h->d_pout);
+  int maxw = 0;
+  for (int l = 1; l < nd.n_layers; l++) maxw = nd.dims[l] > maxw ? nd.dims[l] : maxw;
+  const int o3 = h->pde == PINN_KDV_IDE_DISC ? 1 : 0;        // KdV: the t column block carries u_xxx
+  // per-thread activation arrays sized for the widest hidden layer: the 128-wide instantiation for every net that fits
+  if (maxw <= pinn::MAXW) {
+    if (ns == 1) pinn::mlp_forward_generic<1, pinn::MAXW><<<blocks, threads, 0, h->stream>>>(h->d_w, nd, dx, dt, n, in_dim, h->d_pout, o3);
+    else pinn::mlp_forward_generic<4, pinn::MAXW><<<blocks, threads, 0, h->stream>>>(h->d_w, nd, dx, dt, n, in_dim, h->d_pout, o3);
+  } else {
+    if (ns == 1) pinn::mlp_forward_generic<1, pinn::MAXW_WIDE><<<blocks, threads, 0, h->stream>>>(h->d_w, nd, dx, dt, n, in_dim, h->d_pout, o3);
+    else pinn::mlp_forward_generic<4, pinn::MAXW_WIDE><<<blocks, threads, 0, h->stream>>>(h->d_w, nd, dx, dt, n, in_dim, h->d_pout, o3);
+  }
   CUDA_TRY(cudaGetLastError());
   h->launches++;
   CUDA_TRY(cudaMemcpyAsync(out, h->d_pout, n * no * ns * 8, cudaMemcpyDeviceToHost, h->stream));
@@ -1203,13 +1236,13 @@ int pinn_derivatives(pinn_t* h, const double* X, int64_t n, double* out) {
 
 int64_t pinn_num_residual_points(const pinn_t* h) {
   if (!h) return -1;
-  if (h->pde == PINN_BURGERS_DISC || h->pde == PINN_BURGERS_IDE_DISC) return 0;
+  if (is_disc(h->pde)) return 0;
   return h->pde == PINN_BURGERS_IDE ? h->n_d : h->n_c;
 }
 
 int pinn_residual(pinn_t* h, double* f_out, int64_t n_rows) {
   if (!h || !f_out) return fail("null argument");
-  if (h->pde == PINN_BURGERS_DISC || h->pde == PINN_BURGERS_IDE_DISC) return fail("pinn_residual: not defined for the discrete-time models");
+  if (is_disc(h->pde)) return fail("pinn_residual: not defined for the discrete-time models");
   const bool ide = h->pde == PINN_BURGERS_IDE;
   const int64_t n = ide ? h->n_d : h->n_c;
   if (n_rows != n)

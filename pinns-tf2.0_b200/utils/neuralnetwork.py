@@ -90,7 +90,8 @@ _NATIVE_OVERRIDES = {}
 
 
 class NeuralNetwork(object):
-    pde = None           # optional explicit PDE id: "burgers_inf" | "burgers_ide" | "nls_inf"
+    pde = None           # optional explicit PDE id: "burgers_inf" | "burgers_ide" | "nls_inf" | "burgers_disc" | "burgers_ide_disc"
+    #                      | "kdv_ide_disc" | "ac_disc" (the last two are never guessed from attributes)
     weight_seed = 1234   # stands in for tf.random.set_seed(1234) (inf_cont_burgers.py:10)
 
     def __init_subclass__(cls, **kw):
@@ -159,7 +160,11 @@ class NeuralNetwork(object):
             else:
                 raise pinn_cabi.PinnError("cannot recognise the PDE of %s: set the class attribute `pde`" % type(self).__name__)
         return {"burgers_inf": pinn_cabi.BURGERS_INF, "burgers_ide": pinn_cabi.BURGERS_IDE, "nls_inf": pinn_cabi.NLS_INF,
-                "burgers_disc": pinn_cabi.BURGERS_DISC, "burgers_ide_disc": pinn_cabi.BURGERS_IDE_DISC}[tag]
+                "burgers_disc": pinn_cabi.BURGERS_DISC, "burgers_ide_disc": pinn_cabi.BURGERS_IDE_DISC,
+                "kdv_ide_disc": pinn_cabi.KDV_IDE_DISC, "ac_disc": pinn_cabi.AC_DISC}[tag]
+
+    def _two_snapshots(self):
+        return self._pde_id() in _TWO_SNAPSHOT
 
     def _native(self):
         if self._h is None:
@@ -175,10 +180,14 @@ class NeuralNetwork(object):
                 h.set_pde_params([float(self.nu), float(np.asarray(self.dt).reshape(-1)[0])])
                 h.set_irk(np.asarray(self.IRK_weights, dtype=np.float64))
                 h.set_boundary(np.asarray(self.x_1, dtype=np.float64).reshape(-1))
-            elif pde == pinn_cabi.BURGERS_IDE_DISC:                  # ide_disc_burgers.py:49-55, :151-152
+            elif pde in _TWO_SNAPSHOT:                               # ide_disc_burgers.py:49-55, :151-152 (KdV.py alike)
                 h.set_pde_params([float(np.asarray(self.dt).reshape(-1)[0])])
                 h.set_irk(pinn_cabi.irk_ide_disc(self.IRK_alpha, self.IRK_beta))
                 w = np.concatenate([w, [0.0, -6.0]])
+            elif pde == pinn_cabi.AC_DISC:                           # AC.py: d = 1e-4, k = 5 unless the class sets d / k
+                h.set_pde_params([float(np.asarray(self.dt).reshape(-1)[0]), float(getattr(self, "d", 1e-4)),
+                                  float(getattr(self, "k", 5.0))])
+                h.set_irk(np.asarray(self.IRK_weights, dtype=np.float64))
             elif pde == pinn_cabi.BURGERS_IDE:
                 l1 = float(np.asarray(self.lambda_1.numpy() if hasattr(self.lambda_1, "numpy") else self.lambda_1).reshape(-1)[0])
                 l2 = float(np.asarray(self.lambda_2.numpy() if hasattr(self.lambda_2, "numpy") else self.lambda_2).reshape(-1)[0])
@@ -249,7 +258,7 @@ class NeuralNetwork(object):
 
     def wrap_training_variables(self):
         var = self.model.trainable_variables
-        if self._pde_id() in (pinn_cabi.BURGERS_IDE, pinn_cabi.BURGERS_IDE_DISC):       # ide_cont_burgers.py:93-96
+        if self._pde_id() in (pinn_cabi.BURGERS_IDE,) + _TWO_SNAPSHOT:                 # ide_cont_burgers.py:93-96
             w = self._native().get_weights()
             var = var + [_t(w[-2:-1]), _t(w[-1:])]
         return var
@@ -257,7 +266,7 @@ class NeuralNetwork(object):
     def get_params(self, numpy=False):
         """Base class: no PDE parameters (neuralnetwork.py:64-65); the identification models return (lambda_1, exp(lambda_2))."""
         try:
-            if self._pde_id() in (pinn_cabi.BURGERS_IDE, pinn_cabi.BURGERS_IDE_DISC):
+            if self._pde_id() in (pinn_cabi.BURGERS_IDE,) + _TWO_SNAPSHOT:
                 return _native_get_params(self, numpy)
         except pinn_cabi.PinnError:
             pass
@@ -323,6 +332,10 @@ class NeuralNetwork(object):
         return _t(X)
 
 
+# two-snapshot discrete-time identification models: fit(x_0, u_0, x_1, u_1), predict -> (U_0, U_1), flat vector ends with l1, l2
+_TWO_SNAPSHOT = (pinn_cabi.BURGERS_IDE_DISC, pinn_cabi.KDV_IDE_DISC)
+
+
 # ---------------------------------------------------------------------- native replacements for subclass overrides
 def _native_loss(self, *args):
     """Composite PDE loss of the recognised problem on the bound data (value only)."""
@@ -352,11 +365,15 @@ def _native_f_model(self, *args):
 
 def _ide_disc_models(self, x):
     """U_0 = U + dt N alpha^T and U_1 = U - dt N (beta - alpha)^T on arbitrary points (ide_disc_burgers.py:81-108, predict
-    :197-202): network value and x-derivatives from the device, the two small q x q products on the host (off the step path)."""
+    :197-202): network value and x-derivatives from the device, the two small q x q products on the host (off the step path).
+    Burgers: N = l1 U U_x - e^{l2} U_xx;  KdV: N = l1 U U_x + e^{l2} U_xxx (u_xxx comes in the u_t column block)."""
     n = self._native()
-    U, Ux, _, Uxx = n.derivatives(np.asarray(x, dtype=np.float64).reshape(-1, 1))
+    U, Ux, Uxxx, Uxx = n.derivatives(np.asarray(x, dtype=np.float64).reshape(-1, 1))
     w = n.get_weights()
-    N = w[-2] * U * Ux - np.exp(w[-1]) * Uxx
+    if n.pde == pinn_cabi.KDV_IDE_DISC:
+        N = w[-2] * U * Ux + np.exp(w[-1]) * Uxxx
+    else:
+        N = w[-2] * U * Ux - np.exp(w[-1]) * Uxx
     M = pinn_cabi.irk_ide_disc(self.IRK_alpha, self.IRK_beta)
     q = M.shape[1]
     dt = float(np.asarray(self.dt).reshape(-1)[0])
@@ -364,13 +381,13 @@ def _ide_disc_models(self, x):
 
 
 def _native_U_0_model(self, x, customDummy=None):
-    if self._pde_id() == pinn_cabi.BURGERS_IDE_DISC:
+    if self._two_snapshots():
         return _ide_disc_models(self, x)[0]
     raise pinn_cabi.PinnError("U_0_model is evaluated inside the fused kernel; use grad()/fit()/predict()")
 
 
 def _native_U_1_model(self, x, customDummy=None):
-    if self._pde_id() == pinn_cabi.BURGERS_IDE_DISC:
+    if self._two_snapshots():
         return _ide_disc_models(self, x)[1]
     raise pinn_cabi.PinnError("U_1_model belongs to the discrete-time identification model")
 
@@ -412,13 +429,13 @@ def _native_fit_two_snapshots(self, x_0, u_0, x_1, u_1):
 
 def _two_snapshot_dispatch(name, script_fn):
     def fit(self, *args):
-        if len(args) == 4 and self._pde_id() == pinn_cabi.BURGERS_IDE_DISC:
+        if len(args) == 4 and self._two_snapshots():
             return _native_fit_two_snapshots(self, *args)
         return script_fn(self, *args)
 
     def predict(self, x_star, *rest):
         try:
-            two = self._pde_id() == pinn_cabi.BURGERS_IDE_DISC
+            two = self._two_snapshots()
         except pinn_cabi.PinnError:
             two = False
         if two:
@@ -451,7 +468,7 @@ def _native_get_params(self, numpy=False):
     pde = self._pde_id()
     if pde == pinn_cabi.BURGERS_INF:
         return self.nu
-    if pde in (pinn_cabi.BURGERS_IDE, pinn_cabi.BURGERS_IDE_DISC):
+    if pde in (pinn_cabi.BURGERS_IDE,) + _TWO_SNAPSHOT:
         w = self._native().get_weights()
         l1, l2 = w[-2], np.exp(w[-1])            # ide_cont_burgers.py:109-114, ide_disc_burgers.py:138-143
         return (l1, l2) if numpy else (_t([l1]), _t([l2]))

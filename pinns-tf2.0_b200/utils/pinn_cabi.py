@@ -13,7 +13,7 @@ _HERE = os.path.dirname(os.path.realpath(__file__))
 # PINN_LIB: load another build of the same library (kernel experiments: profiles/kernel_variants.py)
 LIB_PATH = os.environ.get("PINN_LIB") or os.path.join(_HERE, "..", "lib", "libpinn_b200.so")
 
-BURGERS_INF, BURGERS_IDE, NLS_INF, BURGERS_DISC, BURGERS_IDE_DISC = 0, 1, 2, 3, 4
+BURGERS_INF, BURGERS_IDE, NLS_INF, BURGERS_DISC, BURGERS_IDE_DISC, KDV_IDE_DISC, AC_DISC = 0, 1, 2, 3, 4, 5, 6
 LBFGS_REASONS = {0: "running", 1: "max iterations", 2: "max evaluations", 3: "optimality", 4: "step below tolX",
                  5: "f change below tolX", 6: "no progress along direction", 7: "initial optimality"}
 
@@ -162,13 +162,14 @@ class Pinn(object):
         self._ck(self.lib.pinn_set_pde_params(self.h, _p(a), a.size))
 
     def get_params(self):
-        n = {BURGERS_INF: 1, BURGERS_IDE: 2, NLS_INF: 0, BURGERS_DISC: 2, BURGERS_IDE_DISC: 2}[self.pde]
+        n = {BURGERS_INF: 1, BURGERS_IDE: 2, NLS_INF: 0, BURGERS_DISC: 2, BURGERS_IDE_DISC: 2, KDV_IDE_DISC: 2, AC_DISC: 3}[self.pde]
         out = np.zeros(max(n, 1))
         self._ck(self.lib.pinn_get_params(self.h, _p(out), n))
         return out[:n]
 
     def set_irk(self, irk):
-        """BURGERS_DISC: (q+1, q) stage matrix.  BURGERS_IDE_DISC: (2q, q) = [alpha ; -(beta - alpha)] (see irk_ide_disc)."""
+        """BURGERS_DISC, AC_DISC: (q+1, q) stage matrix.  BURGERS_IDE_DISC, KDV_IDE_DISC: (2q, q) = [alpha ; -(beta - alpha)]
+        (see irk_ide_disc)."""
         irk = _arr(irk)
         assert irk.ndim == 2 and irk.shape[0] in (irk.shape[1] + 1, 2 * irk.shape[1])
         self._ck(self.lib.pinn_set_irk(self.h, _p(irk), irk.shape[1]))
