@@ -45,7 +45,12 @@ enum {
                            with u_t + l1 u u_x + exp(l2) u_xxx = 0, i.e. N = l1 U U_x + exp(l2) U_xxx; net [1, ..., q]    */
   PINN_AC_DISC = 6      /* discrete_time_inference (AC)/AC.py of PINNs/main (fp64 restatement): net [1, ..., q+1] on x;
                            N = k U^3 - k U - d U_xx; U_0 = U_1 + dt N IRK^T; loss = sum (U_0 - u_0)^2 + sum over all q+1
-                           outputs of (U_1(lb) - U_1(ub))^2 + (d/dx U_1(lb) - d/dx U_1(ub))^2 (periodic in value and slope) */
+                           outputs of (U_1(lb) - U_1(ub))^2 + (d/dx U_1(lb) - d/dx U_1(ub))^2 (periodic in value and slope) */,
+  PINN_NS_IDE = 7       /* continuous_time_identification (Navier-Stokes)/NavierStokes.py of PINNs/main (fp64 restatement): net
+                           [3, ..., 2] maps (x, y, t) to (psi, p); u = psi_y, v = -psi_x;
+                           f_u = u_t + l1 (u u_x + v u_y) + p_x - l2 (u_xx + u_yy), f_v = v_t + l1 (u v_x + v v_y) + p_y - l2 (v_xx + v_yy);
+                           loss = sum (u - u_d)^2 + sum (v - v_d)^2 + sum f_u^2 + sum f_v^2 over the data points (parts: data, 0,
+                           residual); flat vector ends with the raw [lambda_1, lambda_2]; one GPU only (world == 1)          */
 };
 
 /* L-BFGS stop reasons (utils/custom_lbfgs.py:73-76,154-156,192-215). */
@@ -65,8 +70,9 @@ const char* pinn_version(void);
 
 /* NeuralNetwork.__init__ (utils/neuralnetwork.py:8-47): layers = hp["layers"]; lb/ub feed the normalising
  * Lambda (:29-30).  rank/world/nccl_uid: data-parallel sharding of the collocation set (new capability,
- * SURVEY 8(e)); nccl_uid = 128-byte ncclUniqueId from pinn_nccl_unique_id on rank 0, NULL when world==1. */
-int pinn_create(pinn_t** out, int pde_id, int n_layers, const int* layers, const double lb[2], const double ub[2],
+ * SURVEY 8(e)); nccl_uid = 128-byte ncclUniqueId from pinn_nccl_unique_id on rank 0, NULL when world==1.
+ * lb and ub hold max(2, layers[0]) entries: (x, t), or (x, y, t) for NS_IDE. */
+int pinn_create(pinn_t** out, int pde_id, int n_layers, const int* layers, const double* lb, const double* ub,
                 int device, int rank, int world, const void* nccl_uid);
 int pinn_destroy(pinn_t* h);
 int pinn_nccl_unique_id(void* out128);
@@ -91,7 +97,8 @@ int64_t pinn_num_params(const pinn_t* h);
 int pinn_set_pde_params(pinn_t* h, const double* p, int n);
 /* get_params(numpy=True): BURGERS_INF -> [nu] (inf_cont_burgers.py:92-93); BURGERS_IDE and BURGERS_IDE_DISC ->
  * [lambda_1, exp(lambda_2)] read from the trained flat vector (ide_cont_burgers.py:109-114, ide_disc_burgers.py:138-143);
- * KDV_IDE_DISC -> [lambda_1, exp(lambda_2)] likewise; BURGERS_DISC -> [nu, dt]; AC_DISC -> [dt, d, k]. */
+ * KDV_IDE_DISC -> [lambda_1, exp(lambda_2)] likewise; BURGERS_DISC -> [nu, dt]; AC_DISC -> [dt, d, k];
+ * NS_IDE -> the raw [lambda_1, lambda_2]. */
 int pinn_get_params(pinn_t* h, double* p, int n);
 /* BURGERS_DISC: the implicit Runge-Kutta stage matrix IRK_weights, (q+1) x q row-major (inf_disc_burgers.py:56,86);
  * q+1 must equal the network's output width.
@@ -114,7 +121,9 @@ int pinn_set_collocation_mapped(pinn_t* h, const double* x_pinned, const double*
  * reproduces the Lambda's broadcast of a (N,1) input to (x, t:=x) (quirk Q1, inf_cont_schrodinger.py:164).
  * u is (n,out_dim).  For BURGERS_IDE these are also the residual points (ide_cont_burgers.py:88-91,116-118).
  * weight: 1 on the rank that owns the (replicated) data term, 0 elsewhere.
- * AC_DISC: x_0 (n,1) and u_0 (n,1); the periodic pair is (lb[0], ub[0]) of pinn_create, so it needs no pinn_set_boundary. */
+ * AC_DISC: x_0 (n,1) and u_0 (n,1); the periodic pair is (lb[0], ub[0]) of pinn_create, so it needs no pinn_set_boundary.
+ * NS_IDE: X (n,3) = (x, y, t) and u (n,2) = (u, v); these are also the residual points (no collocation, boundary, stage matrix
+ * or snapshot calls, and no PDE constants). */
 int pinn_set_data(pinn_t* h, const double* X, int64_t n, int in_dim, const double* u, int out_dim, double weight);
 
 /* BURGERS_IDE_DISC and KDV_IDE_DISC: snapshot `which` (0: (x_0,u_0) at t_0, 1: (x_1,u_1) at t_1 = t_0 + dt) of fit(x_0,u_0,x_1,u_1)
@@ -184,14 +193,17 @@ int pinn_lbfgs_feed(pinn_lbfgs_t* s, double f, const double* g, double* x_next, 
 int pinn_lbfgs_f_hist(pinn_lbfgs_t* s, double* f_hist_out, int capacity, int* n_out);
 int pinn_lbfgs_destroy(pinn_lbfgs_t* s);
 
-/* predict (utils/neuralnetwork.py:151-153): forward only on (n,in_dim) points -> (n,out_dim). */
+/* predict (utils/neuralnetwork.py:151-153): forward only on (n,in_dim) points -> (n,out_dim); NS_IDE: (psi, p). */
 int pinn_predict(pinn_t* h, const double* X, int64_t n, int in_dim, double* out);
 /* f_model on the stored residual points (inf_cont_burgers.py:65-90,95-98): the collocation set, or the data points for
  * identification (ide_cont_burgers.py:88-91).  f_out: n_rows * n_res doubles (n_res = 1 Burgers, 2 NLS: f_u then f_v per
- * point); n_rows must equal pinn_num_residual_points(h) -- a mismatch is an error, never a short or long write. */
+ * point; NS_IDE: f_u then f_v per data point); n_rows must equal pinn_num_residual_points(h) -- a mismatch is an error, never
+ * a short or long write. */
 int64_t pinn_num_residual_points(const pinn_t* h);
 int pinn_residual(pinn_t* h, double* f_out, int64_t n_rows);
-/* u, u_x, u_t, u_xx at arbitrary points (parity probes): out is (n, 4*out_dim), [u.., u_x.., u_t.., u_xx..]. */
+/* u, u_x, u_t, u_xx at arbitrary points (parity probes): out is (n, 4*out_dim), [u.., u_x.., u_t.., u_xx..].
+ * NS_IDE: X is (n,3) and out is (n, 13*2): the 13 streams value, x, y, t, xx, xy, yy, xt, yt, xxx, xxy, xyy, yyy in that order,
+ * each block (psi, p). */
 int pinn_derivatives(pinn_t* h, const double* X, int64_t n, double* out);
 
 int pinn_sync(pinn_t* h);

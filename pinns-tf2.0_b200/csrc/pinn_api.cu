@@ -17,6 +17,7 @@
 #include "nls_fused.cuh"
 #include "optim_kernels.cuh"
 #include "generic_fused.cuh"
+#include "navier_stokes_fused.cuh"
 
 namespace {
 
@@ -79,7 +80,7 @@ struct LbfgsGram { double *SY = nullptr, *YY = nullptr, *part = nullptr; int n_c
 struct pinn_handle {
   int pde = 0, device = 0, rank = 0, world = 1;
   std::vector<int> layers;
-  double lb[2] = {0, 0}, ub[2] = {1, 1};
+  double lb[3] = {0, 0, 0}, ub[3] = {1, 1, 1};    // NS_IDE: (x, y, t); the other models use the first two
   int P_net = 0, P = 0;             // net parameters; P = P_net (+2 identification)
   double nu = 0.0, dt = 0.0;        // AC_DISC: nu holds d
   double kc = 0.0;                  // AC_DISC: k
@@ -94,7 +95,7 @@ struct pinn_handle {
   bool tail_inflight = false;   // a launch with the in-kernel tail may still be running on this handle's stream
   pinn::ReduceMap last_map{};       // reduction map / grid / stride of the most recent fused launch
   int last_grid = 0, last_stride = 0;
-  int kernel_kind = 0;              // 0: specialised Burgers DMMA kernel, 1: specialised NLS DMMA kernel, 2: generic
+  int kernel_kind = 0;              // 0: specialised Burgers DMMA kernel, 1: specialised NLS DMMA kernel, 2: generic, 3: Navier-Stokes
   double *d_gH = nullptr, *d_gA = nullptr, *d_gS = nullptr;   // generic kernel scratch
   long long g_pts = 0;
   int burgers_kernel = 2;           // 2: warp-specialised (default); 1: single-role v1 (PINN_BURGERS_KERNEL=v1)
@@ -142,6 +143,10 @@ struct pinn_handle {
   // scratch for predict / derivatives
   double *d_px = nullptr, *d_pout = nullptr;
   long long px_cap = 0, pout_cap = 0;
+  double* d_pscr = nullptr;                 // NS probe: streams of two layers [2][13][maxw][chunk]
+  long long pscr_cap = 0;
+  double* d_nsX = nullptr;                  // NS: training points [n][3] = (x, y, t); targets [n][2] in d_u
+  long long nsx_cap = 0;
 
   ncclComm_t comm = nullptr;
   // NVLink push exchange in the tail of every evaluation (optim_kernels.cuh: exchange_block)
@@ -173,6 +178,7 @@ bool is_nls_net(const std::vector<int>& L) {
 int nls_upload_points(pinn_t* h);
 int nls_launch_eval(pinn_t* h, const int* run_flag);
 int generic_launch_eval(pinn_t* h, const int* run_flag);
+int ns_launch_eval(pinn_t* h, const int* run_flag);
 int disc_upload_points(pinn_t* h);
 
 // One L-BFGS iteration on the device (stop tests of the pending evaluation, history update, direction, step).
@@ -418,6 +424,7 @@ int launch_eval(pinn_t* h, const int* run_flag, bool fused_only = false, const A
   int rc;
   bool tail_done = false;
   if (h->kernel_kind == 2) rc = generic_launch_eval(h, run_flag);
+  else if (h->kernel_kind == 3) rc = ns_launch_eval(h, run_flag);
   else if (h->pde == PINN_BURGERS_INF || h->pde == PINN_BURGERS_IDE) rc = burgers_launch_eval(h, run_flag, ad, fused_only ? nullptr : &tail_done);
   else rc = nls_launch_eval(h, run_flag);
   if (rc) return -1;
@@ -513,6 +520,73 @@ int generic_launch_eval(pinn_t* h, const int* run_flag) {
   map.extra_src[map.n_extra++] = h->P_net + 5;
   map.n_out = map.p_net + map.n_extra;
   h->last_map = map; h->last_grid = grid; h->last_stride = h->pstride;
+  return 0;
+}
+
+// Navier-Stokes identification: every data point also carries the residual term.  A CTA per SM (the kernel is built for one
+// 256-thread CTA per SM), points split evenly; only CTAs that own points are launched.
+int ns_launch_eval(pinn_t* h, const int* run_flag) {
+  namespace S = pinn::nsid;
+  const long long n_total = h->n_d;
+  if (n_total <= 0) return fail("no points set (pinn_set_data)");
+  const long long pts = (n_total + h->n_cta - 1) / h->n_cta;
+  const int grid = (int)((n_total + pts - 1) / pts);
+  pinn::NetDesc nd = net_desc(h);
+  int maxw = 0; long long hsum = 0;
+  for (int l = 0; l < nd.n_layers - 1; l++) { hsum += S::NST * pts * nd.dims[l + 1]; if (nd.dims[l + 1] > maxw) maxw = nd.dims[l + 1]; }
+  const long long a_per = S::NST * pts * maxw;
+  if (pts > h->g_pts) {
+    if (h->d_gH) cudaFree(h->d_gH);
+    if (h->d_gA) cudaFree(h->d_gA);
+    if (h->d_gS) cudaFree(h->d_gS);
+    h->d_gH = h->d_gA = h->d_gS = nullptr;
+    CUDA_TRY(cudaMalloc((void**)&h->d_gH, (size_t)h->n_cta * hsum * 8));
+    CUDA_TRY(cudaMalloc((void**)&h->d_gA, (size_t)h->n_cta * 2 * a_per * 8));
+    CUDA_TRY(cudaMalloc((void**)&h->d_gS, (size_t)h->n_cta * 2 * pts * S::SEEDW * 8));
+    h->g_pts = pts;
+  }
+  S::Args a{};
+  a.w = h->d_w; a.nd = nd;
+  for (int c = 0; c < 3; c++) { a.lb[c] = h->lb[c]; a.sc[c] = 2.0 / (h->ub[c] - h->lb[c]); }
+  a.X = h->d_nsX; a.tgt = h->d_u; a.n_total = n_total; a.p_net = h->P_net;
+  a.scrH = h->d_gH; a.scrA = h->d_gA; a.scrS = h->d_gS;
+  a.h_per_cta = hsum; a.a_per_cta = a_per; a.pts = (int)pts;
+  a.partials = h->d_partials; a.pstride = h->pstride; a.run_flag = run_flag;
+  S::fused_loss_grad<<<grid, S::THREADS, 0, h->stream>>>(a);
+  CUDA_TRY(cudaGetLastError());
+  h->launches++;
+  pinn::ReduceMap map{};
+  map.p_net = h->P_net;
+  map.n_extra = 5;
+  for (int k = 0; k < 5; k++) map.extra_src[k] = h->P_net + k;
+  map.n_out = map.p_net + map.n_extra;
+  h->last_map = map; h->last_grid = grid; h->last_stride = h->pstride;
+  return 0;
+}
+
+// NS probe (pinn_predict / pinn_derivatives / pinn_residual): mode 0 (psi, p), 1 all 13 streams, 2 (f_u, f_v); X is [n][3] on
+// the device.  Chunks of points keep the two-layer stream scratch within 256 MB.
+int ns_probe(pinn_t* h, const double* dX, int64_t n, int mode, double* out_host) {
+  namespace S = pinn::nsid;
+  const int per = mode == 1 ? S::SEEDW : 2;
+  if (ensure(&h->d_pout, &h->pout_cap, n * per)) return -1;
+  pinn::NetDesc nd = net_desc(h);
+  int maxw = 1;
+  for (int l = 1; l < nd.n_layers; l++) maxw = nd.dims[l] > maxw ? nd.dims[l] : maxw;
+  long long chunk = (32LL << 20) / (2LL * S::NST * maxw);
+  if (chunk > n) chunk = n;
+  if (ensure(&h->d_pscr, &h->pscr_cap, 2LL * S::NST * maxw * chunk)) return -1;
+  S::Probe pr{};
+  for (int c = 0; c < 3; c++) { pr.lb[c] = h->lb[c]; pr.sc[c] = 2.0 / (h->ub[c] - h->lb[c]); }
+  pr.p_net = h->P_net; pr.maxw = maxw; pr.mode = mode; pr.chunk = chunk;
+  for (long long c0 = 0; c0 < n; c0 += chunk) {
+    const long long m = n - c0 < chunk ? n - c0 : chunk;
+    S::probe_forward<<<(int)((m + 127) / 128), 128, 0, h->stream>>>(h->d_w, nd, pr, dX + 3 * c0, m, h->d_pout + per * c0, h->d_pscr);
+    CUDA_TRY(cudaGetLastError());
+    h->launches++;
+  }
+  CUDA_TRY(cudaMemcpyAsync(out_host, h->d_pout, n * per * 8, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(cudaStreamSynchronize(h->stream));
   return 0;
 }
 
@@ -658,11 +732,13 @@ int pinn_nccl_unique_id(void* out128) {
   return 0;
 }
 
-int pinn_create(pinn_t** out, int pde_id, int n_layers, const int* layers, const double lb[2], const double ub[2],
+int pinn_create(pinn_t** out, int pde_id, int n_layers, const int* layers, const double* lb, const double* ub,
                 int device, int rank, int world, const void* nccl_uid) {
   if (!out || !layers || !lb || !ub) return fail("pinn_create: null argument");
   if (n_layers < 3 || n_layers > pinn::MAXL) return fail("pinn_create: need 3..16 layer sizes");
-  if (pde_id < 0 || pde_id > 6) return fail("pinn_create: unknown pde_id");
+  if (pde_id < 0 || pde_id > 7) return fail("pinn_create: unknown pde_id");
+  const bool ns = pde_id == PINN_NS_IDE;
+  if (ns && world > 1) return fail("pinn_create: the Navier-Stokes identification model runs on one GPU (world must be 1)");
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
     return fail("pinn_create: no CUDA device -- this library has no CPU fallback");
@@ -676,15 +752,22 @@ int pinn_create(pinn_t** out, int pde_id, int n_layers, const int* layers, const
     const int cap = (disc && i == n_layers - 1) ? 512 : pinn::MAXW_WIDE;     // the IRK head may be q+1 = 501 wide
     if (v < 1 || v > cap) { delete h; return fail("pinn_create: layer width out of range (1..256; IRK head <= 512)"); }
   }
-  if (h->layers[0] != (disc ? 1 : 2)) {
+  if (ns) {
+    if (h->layers[0] != 3 || h->layers.back() != 2) {
+      delete h;
+      return fail("pinn_create: the Navier-Stokes identification model needs a net [3, ..., 2]: (x, y, t) -> (psi, p)");
+    }
+  } else if (h->layers[0] != (disc ? 1 : 2)) {
     delete h;
     return fail(disc ? "pinn_create: the discrete-time model takes a 1-D input (x)" : "pinn_create: input dimension must be 2 (x,t)");
   }
   h->lb[0] = lb[0]; h->ub[0] = ub[0];
   h->lb[1] = disc ? 0.0 : lb[1]; h->ub[1] = disc ? 1.0 : ub[1];            // the t axis does not exist for 1-D nets
-  if (!(h->ub[0] > h->lb[0]) || !(h->ub[1] > h->lb[1])) { delete h; return fail("pinn_create: need ub > lb"); }
+  if (ns) { h->lb[2] = lb[2]; h->ub[2] = ub[2]; }
+  if (!(h->ub[0] > h->lb[0]) || !(h->ub[1] > h->lb[1]) || !(h->ub[2] > h->lb[2])) { delete h; return fail("pinn_create: need ub > lb"); }
   const int want_out = pde_id == PINN_NLS_INF ? 2 : 1;
-  if (is_ide_disc(pde_id)) {
+  if (ns) {
+  } else if (is_ide_disc(pde_id)) {
     if (h->layers.back() < 1) { delete h; return fail("pinn_create: the discrete-time identification model needs q >= 1 outputs"); }
   } else if (disc) {
     if (h->layers.back() < 2) { delete h; return fail("pinn_create: the discrete-time model needs q+1 >= 2 outputs"); }
@@ -698,11 +781,11 @@ int pinn_create(pinn_t** out, int pde_id, int n_layers, const int* layers, const
     const char* fg = getenv("PINN_FORCE_GENERIC");
     const bool force = fg && fg[0] == '1';
     const bool special = disc ? false : ((pde_id == PINN_NLS_INF) ? is_nls_net(h->layers) : is_burgers_net(h->layers));
-    h->kernel_kind = (special && !force) ? (pde_id == PINN_NLS_INF ? 1 : 0) : 2;
+    h->kernel_kind = ns ? 3 : (special && !force) ? (pde_id == PINN_NLS_INF ? 1 : 0) : 2;
   }
   h->P_net = 0;
   for (int l = 0; l + 1 < n_layers; l++) h->P_net += layers[l] * layers[l + 1] + layers[l + 1];
-  h->P = h->P_net + ((pde_id == PINN_BURGERS_IDE || is_ide_disc(pde_id)) ? 2 : 0);
+  h->P = h->P_net + ((pde_id == PINN_BURGERS_IDE || is_ide_disc(pde_id) || ns) ? 2 : 0);
 
 #define CREATE_TRY(expr)                                                                          \
   do {                                                                                            \
@@ -742,7 +825,10 @@ int pinn_create(pinn_t** out, int pde_id, int n_layers, const int* layers, const
   CREATE_TRY(cudaMemset(h->d_loss_ring, 0, LOSS_RING * 8));
   CREATE_TRY(cudaMalloc((void**)&h->d_lb, sizeof(pinn::LbfgsState)));
   CREATE_TRY(cudaMemset(h->d_lb, 0, sizeof(pinn::LbfgsState)));
-  if (h->kernel_kind == 2) {
+  if (h->kernel_kind == 3) {
+    h->n_cta = h->n_sm;
+    h->pstride = ((h->P_net + 8 + 15) / 16) * 16;
+  } else if (h->kernel_kind == 2) {
     h->n_cta = 2 * h->n_sm;
     h->pstride = ((h->P_net + 8 + 15) / 16) * 16;
   } else if (pde_id == PINN_NLS_INF) {
@@ -788,7 +874,7 @@ int pinn_destroy(pinn_t* h) {
   if (h->d_xseq) cudaFree(h->d_xseq);
   if (h->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(h->comm);
   double* bufs[] = {h->d_w, h->d_R, h->d_partials, h->d_m, h->d_v, h->d_loss_ring, h->d_x, h->d_t, h->d_u, h->d_scrH, h->d_scrA, h->d_scrS, h->d_gH, h->d_gA, h->d_gS, h->d_irk, h->d_gold,
-                    h->d_d, h->d_S, h->d_Y, h->d_xfinal, h->d_fhist, h->d_px, h->d_pout};
+                    h->d_d, h->d_S, h->d_Y, h->d_xfinal, h->d_fhist, h->d_px, h->d_pout, h->d_pscr, h->d_nsX};
   for (double* b : bufs) if (b) cudaFree(b);
   if (h->d_step) cudaFree(h->d_step);
   if (h->d_lb) cudaFree(h->d_lb);
@@ -847,6 +933,13 @@ int pinn_get_params(pinn_t* h, double* p, int n) {
     p[0] = lam[0]; p[1] = std::exp(lam[1]);         // ide_cont_burgers.py:109-114, ide_disc_burgers.py:138-143
     return 0;
   }
+  if (h->pde == PINN_NS_IDE) {
+    if (n != 2) return fail("pinn_get_params: NS_IDE has two parameters (lambda_1, lambda_2)");
+    CUDA_TRY(cudaSetDevice(h->device));
+    CUDA_TRY(cudaMemcpyAsync(p, h->d_w + h->P_net, 16, cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(cudaStreamSynchronize(h->stream));
+    return 0;
+  }
   if (h->pde == PINN_BURGERS_DISC) {
     if (n != 2) return fail("pinn_get_params: BURGERS_DISC has two constants (nu, dt)");
     p[0] = h->nu; p[1] = h->dt;
@@ -879,7 +972,8 @@ int pinn_set_irk(pinn_t* h, const double* irk, int q) {
 
 int pinn_set_collocation(pinn_t* h, const double* x, const double* t, int64_t n, int64_t n_global) {
   if (!h) return fail("null handle");
-  if (h->pde == PINN_BURGERS_IDE) return fail("pinn_set_collocation: identification uses the data points as residual points");
+  if (h->pde == PINN_BURGERS_IDE || h->pde == PINN_NS_IDE)
+    return fail("pinn_set_collocation: identification uses the data points as residual points");
   if (is_disc(h->pde))
     return fail("pinn_set_collocation: the discrete-time models have no collocation set (snapshot / boundary points only)");
   if (n < 0 || (n > 0 && (!x || !t))) return fail("pinn_set_collocation: bad arguments");
@@ -919,6 +1013,19 @@ int pinn_set_collocation_mapped(pinn_t* h, const double* x_pinned, const double*
 int pinn_set_data(pinn_t* h, const double* X, int64_t n, int in_dim, const double* u, int out_dim, double weight) {
   if (!h) return fail("null handle");
   if (n < 0 || (n > 0 && (!X || !u))) return fail("pinn_set_data: bad arguments");
+  if (h->pde == PINN_NS_IDE) {
+    // X (n,3) = (x, y, t), u (n,2) = (u, v); these points also carry the residual term
+    if (in_dim != 3 || out_dim != 2) return fail("pinn_set_data: the Navier-Stokes model takes X (n,3) = (x, y, t) and u (n,2) = (u, v)");
+    CUDA_TRY(cudaSetDevice(h->device));
+    if (n) {
+      if (ensure(&h->d_nsX, &h->nsx_cap, 3 * n) || ensure(&h->d_u, &h->u_cap, 2 * n)) return -1;
+      CUDA_TRY(cudaMemcpyAsync(h->d_nsX, X, n * 3 * 8, cudaMemcpyHostToDevice, h->stream));
+      CUDA_TRY(cudaMemcpyAsync(h->d_u, u, n * 2 * 8, cudaMemcpyHostToDevice, h->stream));
+      CUDA_TRY(cudaStreamSynchronize(h->stream));
+    }
+    h->n_d = n; h->d_out_dim = 2; h->data_weight = weight;
+    return 0;
+  }
   if (in_dim != 1 && in_dim != 2) return fail("pinn_set_data: in_dim must be 1 (broadcast quirk) or 2");
   if (is_ide_disc(h->pde)) return pinn_set_snapshot(h, 0, X, n, u);
   if (h->pde == PINN_BURGERS_DISC || h->pde == PINN_AC_DISC) {
@@ -1226,23 +1333,44 @@ static int forward_generic(pinn_t* h, const double* X, const double* dx, const d
   return 0;
 }
 
+// NS handles: the probe kernel on host points X (n,3)
+static int forward_ns(pinn_t* h, const double* X, int64_t n, int in_dim, double* out, int mode) {
+  if (!h || !out || !X) return fail("null argument");
+  if (in_dim != 3) return fail("the Navier-Stokes model takes X (n,3) = (x, y, t)");
+  if (n <= 0) return 0;
+  CUDA_TRY(cudaSetDevice(h->device));
+  if (ensure(&h->d_px, &h->px_cap, n * 3)) return -1;
+  CUDA_TRY(cudaMemcpyAsync(h->d_px, X, n * 3 * 8, cudaMemcpyHostToDevice, h->stream));
+  return ns_probe(h, h->d_px, n, mode, out);
+}
+
 int pinn_predict(pinn_t* h, const double* X, int64_t n, int in_dim, double* out) {
+  if (h && h->pde == PINN_NS_IDE) return forward_ns(h, X, n, in_dim, out, 0);
   return forward_generic(h, X, nullptr, nullptr, n, in_dim, out, 1);
 }
 
 int pinn_derivatives(pinn_t* h, const double* X, int64_t n, double* out) {
+  if (h && h->pde == PINN_NS_IDE) return forward_ns(h, X, n, 3, out, 1);
   return forward_generic(h, X, nullptr, nullptr, n, h ? h->layers[0] : 2, out, 4);
 }
 
 int64_t pinn_num_residual_points(const pinn_t* h) {
   if (!h) return -1;
   if (is_disc(h->pde)) return 0;
-  return h->pde == PINN_BURGERS_IDE ? h->n_d : h->n_c;
+  return (h->pde == PINN_BURGERS_IDE || h->pde == PINN_NS_IDE) ? h->n_d : h->n_c;
 }
 
 int pinn_residual(pinn_t* h, double* f_out, int64_t n_rows) {
   if (!h || !f_out) return fail("null argument");
   if (is_disc(h->pde)) return fail("pinn_residual: not defined for the discrete-time models");
+  if (h->pde == PINN_NS_IDE) {
+    if (n_rows != h->n_d)
+      return fail("pinn_residual: the output buffer holds " + std::to_string(n_rows) + " rows but " + std::to_string(h->n_d) +
+                  " residual points are stored (pinn_num_residual_points)");
+    if (h->n_d == 0) return 0;
+    CUDA_TRY(cudaSetDevice(h->device));
+    return ns_probe(h, h->d_nsX, h->n_d, 2, f_out);
+  }
   const bool ide = h->pde == PINN_BURGERS_IDE;
   const int64_t n = ide ? h->n_d : h->n_c;
   if (n_rows != n)
@@ -1360,7 +1488,10 @@ int pinn_kernel_info(pinn_t* h, char* buf, int buflen) {
   if (!h || !buf || buflen < 1) return fail("bad arguments");
   cudaFuncAttributes fa{};
   int smem = 0, threads = 0;
-  if (h->kernel_kind == 2) {
+  if (h->kernel_kind == 3) {
+    CUDA_TRY(cudaFuncGetAttributes(&fa, pinn::nsid::fused_loss_grad));
+    smem = 0; threads = pinn::nsid::THREADS;
+  } else if (h->kernel_kind == 2) {
     CUDA_TRY(cudaFuncGetAttributes(&fa, pinn::generic::fused_loss_grad));
     smem = 0; threads = pinn::generic::THREADS;
   } else if (h->pde == PINN_NLS_INF) {

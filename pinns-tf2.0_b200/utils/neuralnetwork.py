@@ -91,7 +91,7 @@ _NATIVE_OVERRIDES = {}
 
 class NeuralNetwork(object):
     pde = None           # optional explicit PDE id: "burgers_inf" | "burgers_ide" | "nls_inf" | "burgers_disc" | "burgers_ide_disc"
-    #                      | "kdv_ide_disc" | "ac_disc" (the last two are never guessed from attributes)
+    #                      | "kdv_ide_disc" | "ac_disc" | "ns_ide" (the last three are never guessed from attributes)
     weight_seed = 1234   # stands in for tf.random.set_seed(1234) (inf_cont_burgers.py:10)
 
     def __init_subclass__(cls, **kw):
@@ -161,7 +161,7 @@ class NeuralNetwork(object):
                 raise pinn_cabi.PinnError("cannot recognise the PDE of %s: set the class attribute `pde`" % type(self).__name__)
         return {"burgers_inf": pinn_cabi.BURGERS_INF, "burgers_ide": pinn_cabi.BURGERS_IDE, "nls_inf": pinn_cabi.NLS_INF,
                 "burgers_disc": pinn_cabi.BURGERS_DISC, "burgers_ide_disc": pinn_cabi.BURGERS_IDE_DISC,
-                "kdv_ide_disc": pinn_cabi.KDV_IDE_DISC, "ac_disc": pinn_cabi.AC_DISC}[tag]
+                "kdv_ide_disc": pinn_cabi.KDV_IDE_DISC, "ac_disc": pinn_cabi.AC_DISC, "ns_ide": pinn_cabi.NS_IDE}[tag]
 
     def _two_snapshots(self):
         return self._pde_id() in _TWO_SNAPSHOT
@@ -188,6 +188,8 @@ class NeuralNetwork(object):
                 h.set_pde_params([float(np.asarray(self.dt).reshape(-1)[0]), float(getattr(self, "d", 1e-4)),
                                   float(getattr(self, "k", 5.0))])
                 h.set_irk(np.asarray(self.IRK_weights, dtype=np.float64))
+            elif pde == pinn_cabi.NS_IDE:                            # NavierStokes.py: raw lambdas, both 0.0 unless the class sets them
+                w = np.concatenate([w, [_scalar(getattr(self, "lambda_1", 0.0)), _scalar(getattr(self, "lambda_2", 0.0))]])
             elif pde == pinn_cabi.BURGERS_IDE:
                 l1 = float(np.asarray(self.lambda_1.numpy() if hasattr(self.lambda_1, "numpy") else self.lambda_1).reshape(-1)[0])
                 l2 = float(np.asarray(self.lambda_2.numpy() if hasattr(self.lambda_2, "numpy") else self.lambda_2).reshape(-1)[0])
@@ -258,15 +260,16 @@ class NeuralNetwork(object):
 
     def wrap_training_variables(self):
         var = self.model.trainable_variables
-        if self._pde_id() in (pinn_cabi.BURGERS_IDE,) + _TWO_SNAPSHOT:                 # ide_cont_burgers.py:93-96
+        if self._pde_id() in _LAMBDAS:                                                # ide_cont_burgers.py:93-96
             w = self._native().get_weights()
             var = var + [_t(w[-2:-1]), _t(w[-1:])]
         return var
 
     def get_params(self, numpy=False):
-        """Base class: no PDE parameters (neuralnetwork.py:64-65); the identification models return (lambda_1, exp(lambda_2))."""
+        """Base class: no PDE parameters (neuralnetwork.py:64-65); the identification models return (lambda_1, exp(lambda_2)),
+        Navier-Stokes the raw (lambda_1, lambda_2)."""
         try:
-            if self._pde_id() in (pinn_cabi.BURGERS_IDE,) + _TWO_SNAPSHOT:
+            if self._pde_id() in _LAMBDAS:
                 return _native_get_params(self, numpy)
         except pinn_cabi.PinnError:
             pass
@@ -323,7 +326,19 @@ class NeuralNetwork(object):
         self.logger.log_train_end(self.tf_epochs + self.nt_config.maxIter)
 
     def predict(self, X_star):
+        if self._is_ns():
+            return _ns_fields(self, X_star)[:3]
         return self.model(X_star).numpy()
+
+    def f_model(self, X=None):
+        """Residuals on the stored residual points (Navier-Stokes: (f_u, f_v), or on the points X when given)."""
+        return _native_f_model(self, *(() if X is None else (X,)))
+
+    def _is_ns(self):
+        try:
+            return self._pde_id() == pinn_cabi.NS_IDE
+        except pinn_cabi.PinnError:
+            return False
 
     def summary(self):
         return self.model.summary()
@@ -334,6 +349,25 @@ class NeuralNetwork(object):
 
 # two-snapshot discrete-time identification models: fit(x_0, u_0, x_1, u_1), predict -> (U_0, U_1), flat vector ends with l1, l2
 _TWO_SNAPSHOT = (pinn_cabi.BURGERS_IDE_DISC, pinn_cabi.KDV_IDE_DISC)
+# every model whose flat vector ends with [lambda_1, lambda_2]
+_LAMBDAS = (pinn_cabi.BURGERS_IDE, pinn_cabi.NS_IDE) + _TWO_SNAPSHOT
+
+
+def _scalar(v):
+    return float(np.asarray(v.numpy() if hasattr(v, "numpy") else v, dtype=np.float64).reshape(-1)[0])
+
+
+def _ns_fields(self, X):
+    """Navier-Stokes (u, v, p, f_u, f_v) on the points X (N,3), each (N,1), from the 13 device streams of (psi, p):
+    u = psi_y, v = -psi_x (NavierStokes.py net_NS)."""
+    n = self._native()
+    D = n.derivatives(np.asarray(X, dtype=np.float64))
+    l1, l2 = n.get_weights()[-2:]
+    P, Q = D[:, :, 0], D[:, :, 1]
+    px, py, pxx, pxy, pyy = P[:, 1], P[:, 2], P[:, 4], P[:, 5], P[:, 6]
+    f_u = P[:, 8] + l1 * (py * pxy - px * pyy) + Q[:, 1] - l2 * (P[:, 10] + P[:, 12])
+    f_v = -P[:, 7] + l1 * (px * pxy - py * pxx) + Q[:, 2] + l2 * (P[:, 9] + P[:, 11])
+    return tuple(_t(a[:, None]) for a in (py, -px, Q[:, 0], f_u, f_v))
 
 
 # ---------------------------------------------------------------------- native replacements for subclass overrides
@@ -349,6 +383,8 @@ def _native_f_model(self, *args):
     """f_model (inf_cont_burgers.py:65-90 / ide_cont_burgers.py:56-85 / inf_cont_schrodinger.py:79-105): on the stored
     residual points, or -- identification, where the reference passes the points explicitly -- on the given points."""
     n = self._native()
+    if self._pde_id() == pinn_cabi.NS_IDE and args:
+        return _ns_fields(self, args[0])[3:]
     if self._pde_id() == pinn_cabi.BURGERS_IDE:
         if args:
             U, Ux, Ut, Uxx = n.derivatives(np.asarray(args[0], dtype=np.float64))
@@ -440,6 +476,8 @@ def _two_snapshot_dispatch(name, script_fn):
             two = False
         if two:
             return _ide_disc_models(self, x_star)
+        if self._is_ns():
+            return _ns_fields(self, x_star)[:3]
         return script_fn(self, x_star, *rest)
 
     fn = fit if name == "fit" else predict
@@ -468,6 +506,9 @@ def _native_get_params(self, numpy=False):
     pde = self._pde_id()
     if pde == pinn_cabi.BURGERS_INF:
         return self.nu
+    if pde == pinn_cabi.NS_IDE:
+        l1, l2 = self._native().get_weights()[-2:]     # raw lambdas (NavierStokes.py)
+        return (l1, l2) if numpy else (_t([l1]), _t([l2]))
     if pde in (pinn_cabi.BURGERS_IDE,) + _TWO_SNAPSHOT:
         w = self._native().get_weights()
         l1, l2 = w[-2], np.exp(w[-1])            # ide_cont_burgers.py:109-114, ide_disc_burgers.py:138-143

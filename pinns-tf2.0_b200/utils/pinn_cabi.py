@@ -13,7 +13,9 @@ _HERE = os.path.dirname(os.path.realpath(__file__))
 # PINN_LIB: load another build of the same library (kernel experiments: profiles/kernel_variants.py)
 LIB_PATH = os.environ.get("PINN_LIB") or os.path.join(_HERE, "..", "lib", "libpinn_b200.so")
 
-BURGERS_INF, BURGERS_IDE, NLS_INF, BURGERS_DISC, BURGERS_IDE_DISC, KDV_IDE_DISC, AC_DISC = 0, 1, 2, 3, 4, 5, 6
+BURGERS_INF, BURGERS_IDE, NLS_INF, BURGERS_DISC, BURGERS_IDE_DISC, KDV_IDE_DISC, AC_DISC, NS_IDE = 0, 1, 2, 3, 4, 5, 6, 7
+# Navier-Stokes derivative streams, in the order of pinn_derivatives' blocks
+NS_STREAMS = ("u", "x", "y", "t", "xx", "xy", "yy", "xt", "yt", "xxx", "xxy", "xyy", "yyy")
 LBFGS_REASONS = {0: "running", 1: "max iterations", 2: "max evaluations", 3: "optimality", 4: "step below tolX",
                  5: "f change below tolX", 6: "no progress along direction", 7: "initial optimality"}
 
@@ -162,7 +164,8 @@ class Pinn(object):
         self._ck(self.lib.pinn_set_pde_params(self.h, _p(a), a.size))
 
     def get_params(self):
-        n = {BURGERS_INF: 1, BURGERS_IDE: 2, NLS_INF: 0, BURGERS_DISC: 2, BURGERS_IDE_DISC: 2, KDV_IDE_DISC: 2, AC_DISC: 3}[self.pde]
+        n = {BURGERS_INF: 1, BURGERS_IDE: 2, NLS_INF: 0, BURGERS_DISC: 2, BURGERS_IDE_DISC: 2, KDV_IDE_DISC: 2, AC_DISC: 3,
+             NS_IDE: 2}[self.pde]
         out = np.zeros(max(n, 1))
         self._ck(self.lib.pinn_get_params(self.h, _p(out), n))
         return out[:n]
@@ -271,8 +274,12 @@ class Pinn(object):
         return out
 
     def derivatives(self, X):
-        """(u, u_x, u_t, u_xx), each (n, out_dim)."""
+        """(u, u_x, u_t, u_xx), each (n, out_dim).  NS_IDE: one (n, 13, 2) array, the streams of NS_STREAMS, each (psi, p)."""
         X = _arr(X)
+        if self.pde == NS_IDE:
+            out = np.empty((X.shape[0], len(NS_STREAMS), 2))
+            self._ck(self.lib.pinn_derivatives(self.h, _p(X), X.shape[0], _p(out)))
+            return out
         out = np.empty((X.shape[0], 4, self.out_dim))
         self._ck(self.lib.pinn_derivatives(self.h, _p(X), X.shape[0], _p(out)))
         return out[:, 0], out[:, 1], out[:, 2], out[:, 3]
@@ -280,7 +287,7 @@ class Pinn(object):
     def residual(self, n=None):
         """f_model on the stored residual points.  The buffer is sized from the count the handle holds; a caller-supplied
         `n` is only checked against it."""
-        nres = 2 if self.pde == NLS_INF else 1
+        nres = 2 if self.pde in (NLS_INF, NS_IDE) else 1
         stored = int(self.lib.pinn_num_residual_points(self.h))
         if n is not None and int(n) != stored:
             raise PinnError(f"residual: {stored} residual points are stored, caller expected {int(n)}")
