@@ -50,7 +50,13 @@ enum {
                            [3, ..., 2] maps (x, y, t) to (psi, p); u = psi_y, v = -psi_x;
                            f_u = u_t + l1 (u u_x + v u_y) + p_x - l2 (u_xx + u_yy), f_v = v_t + l1 (u v_x + v v_y) + p_y - l2 (v_xx + v_yy);
                            loss = sum (u - u_d)^2 + sum (v - v_d)^2 + sum f_u^2 + sum f_v^2 over the data points (parts: data, 0,
-                           residual); flat vector ends with the raw [lambda_1, lambda_2]; one GPU only (world == 1)          */
+                           residual); flat vector ends with the raw [lambda_1, lambda_2]; one GPU only (world == 1)          */,
+  PINN_POLY_INF = 8,    /* user-defined residual (pinn_set_residual) on a net [2, ..., 1]:
+                           f = sum_k c_k kappa_k u^a_k u_x^b_k u_t^c_k u_xx^d_k - s(x, t); every kappa_k = 1;
+                           loss structure of BURGERS_INF (data term of pinn_set_data + mean f^2 over pinn_set_collocation)  */
+  PINN_POLY_IDE = 9     /* as POLY_INF with kappa_k in {1, l1, l2, e^l1, e^l2}; loss structure of BURGERS_IDE (the residual on the
+                           data points); flat vector ends with the raw [lambda_1, lambda_2].  Both poly ids run on the generic
+                           fused kernel and on one GPU only (world == 1)                                                    */
 };
 
 /* L-BFGS stop reasons (utils/custom_lbfgs.py:73-76,154-156,192-215). */
@@ -98,7 +104,7 @@ int pinn_set_pde_params(pinn_t* h, const double* p, int n);
 /* get_params(numpy=True): BURGERS_INF -> [nu] (inf_cont_burgers.py:92-93); BURGERS_IDE and BURGERS_IDE_DISC ->
  * [lambda_1, exp(lambda_2)] read from the trained flat vector (ide_cont_burgers.py:109-114, ide_disc_burgers.py:138-143);
  * KDV_IDE_DISC -> [lambda_1, exp(lambda_2)] likewise; BURGERS_DISC -> [nu, dt]; AC_DISC -> [dt, d, k];
- * NS_IDE -> the raw [lambda_1, lambda_2]. */
+ * NS_IDE and POLY_IDE -> the raw [lambda_1, lambda_2]. */
 int pinn_get_params(pinn_t* h, double* p, int n);
 /* BURGERS_DISC: the implicit Runge-Kutta stage matrix IRK_weights, (q+1) x q row-major (inf_disc_burgers.py:56,86);
  * q+1 must equal the network's output width.
@@ -129,6 +135,16 @@ int pinn_set_data(pinn_t* h, const double* X, int64_t n, int in_dim, const doubl
 /* BURGERS_IDE_DISC and KDV_IDE_DISC: snapshot `which` (0: (x_0,u_0) at t_0, 1: (x_1,u_1) at t_1 = t_0 + dt) of fit(x_0,u_0,x_1,u_1)
  * (ide_disc_burgers.py:149-156); x and u are (n,1), u broadcasts over the q stages.  pinn_set_data == snapshot 0. */
 int pinn_set_snapshot(pinn_t* h, int which, const double* x, int64_t n, const double* u);
+
+/* POLY_INF / POLY_IDE: the residual f = sum_k coef[k] kappa_k u^e0 u_x^e1 u_t^e2 u_xx^e3 - s.  n_terms in 1..16; exps is
+ * n_terms x 4 row-major in the order (u, u_x, u_t, u_xx), each 0..3, no all-zero row; kind[k] in 0..4 selects kappa_k =
+ * 1, lambda_1, lambda_2, exp(lambda_1), exp(lambda_2) (raw trainable lambdas; POLY_INF takes kind 0 only); coef finite.  The
+ * spec may be replaced at any time; evaluating a poly handle before it is set is an error. */
+int pinn_set_residual(pinn_t* h, int n_terms, const double* coef, const int* kind, const int* exps);
+/* POLY_INF / POLY_IDE: the source s at the stored residual points, n == pinn_num_residual_points(h).  Storing new residual
+ * points (pinn_set_collocation for POLY_INF, pinn_set_data for POLY_IDE) resets the source to zero, so a source never
+ * outlives the points it was computed for. */
+int pinn_set_source(pinn_t* h, const double* s, int64_t n);
 
 /* NLS periodic-boundary times tb (N_b,1): X_lb=(lb0,tb), X_ub=(ub0,tb) (inf_cont_schrodinger.py:50-53).
  * BURGERS_DISC: the boundary positions x_1 on which sum(net(x_1)^2) is imposed (inf_disc_burgers.py:57,99). */

@@ -1,7 +1,8 @@
 // Generic fused PINN loss + gradient kernel: ANY tanh MLP [2, w_1, ..., w_k, out] (hidden widths <= 256, <= 15 Dense layers),
 // PDE heads: Burgers inference / identification (out = 1), Schrodinger (out = 2), and the discrete-time (implicit
 // Runge-Kutta) models on 1-D nets [1, ..., q(+1)] (q+1 <= 512 outputs): Burgers inference and identification
-// (1d-burgers/inf_disc_burgers.py, ide_disc_burgers.py), KdV identification and Allen-Cahn inference; fp64, sm_90a.
+// (1d-burgers/inf_disc_burgers.py, ide_disc_burgers.py), KdV identification and Allen-Cahn inference; and, in the POLY
+// instantiation, a user-defined polynomial residual in (u, u_x, u_t, u_xx) on nets [2, ..., 1] (pde 8, 9); fp64, sm_90a.
 //
 // Purpose: hp["layers"] is user-configurable in the reference (1d-burgers/inf_cont_burgers.py:23-34); the DMMA kernels
 // (burgers_fused_v2.cuh, nls_fused.cuh) are specialised for the two BASELINE nets.  This kernel keeps the path a drop-in
@@ -26,6 +27,15 @@ namespace generic {
 
 constexpr int THREADS = 256;
 constexpr int MAXOUT = 2;
+constexpr int POLY_MAXT = 16;
+
+// A polynomial residual (pinn_set_residual): term k is coef[k] * kappa * u^e0 u_x^e1 u_t^e2 u_xx^e3 with
+// code[k] = kind | e0 << 3 | e1 << 5 | e2 << 7 | e3 << 9, kind 0..4 selecting kappa = 1, l1, l2, e^l1, e^l2 (raw lambdas).
+struct PolySpec {
+  int n;
+  int code[POLY_MAXT];
+  double coef[POLY_MAXT];
+};
 
 struct Args {
   const double* w;
@@ -35,7 +45,7 @@ struct Args {
   const double* tgt;          // data targets [n_d][out]
   long long n_total;
   int pde;                    // PINN_BURGERS_INF / PINN_BURGERS_IDE / PINN_NLS_INF / PINN_BURGERS_DISC (3) / PINN_BURGERS_IDE_DISC (4)
-                              // / PINN_KDV_IDE_DISC (5) / PINN_AC_DISC (6)
+                              // / PINN_KDV_IDE_DISC (5) / PINN_AC_DISC (6) / PINN_POLY_INF (8) / PINN_POLY_IDE (9)
   int in_dim;                 // 2 (x,t), or 1 (x only: discrete-time models)
   int o3;                     // third-order mode: the t slot carries the xxx stream (KdV)
   double dt;                  // DISC, AC: time step;  irk: (q+1) x q stage matrix, q = out - 1;  IDE_DISC, KdV: [M_0 ; M_1], each q x q, q = out
@@ -57,7 +67,20 @@ struct Args {
   double* partials;           // [grid][pstride]: [grad p_net | dl1 dl2 - part0 part1 part2]
   int pstride;
   const int* run_flag;
+  // PINN_POLY_INF (8) / PINN_POLY_IDE (9), read only by fused_loss_grad<true>: the residual's term table, and the source s at
+  // the residual points [n_c] (nullptr: s = 0)
+  PolySpec poly;
+  const double* src;
 };
+
+// Polynomial residual head (DESIGN 4.4d): f = sum_k c_k kappa_k u^a u_x^b u_t^c u_xx^d - s.  A stream's power v^e and its
+// derivative e v^(e-1) are picked from the powers formed once per point, never by dividing by v (u may be 0).
+__device__ __forceinline__ double pick_pow(double v, double v2, double v3, int e) {
+  return e == 0 ? 1.0 : (e == 1 ? v : (e == 2 ? v2 : v3));
+}
+__device__ __forceinline__ double pick_dpow(double v, double v2, int e) {
+  return e == 0 ? 0.0 : (e == 1 ? 1.0 : (e == 2 ? 2.0 * v : 3.0 * v2));
+}
 
 // ---- DMMA.8x8x4 building block for the hidden layers: operands straight from global memory (the per-CTA scratch is L1/L2
 // resident, the weights come through the read-only path); no shared-memory staging, so it works for any width.
@@ -275,6 +298,9 @@ __device__ __noinline__ HeadSums disc_head(const DiscArgs p, int npts, int out, 
   return {part0, part1, gl1, gl2};
 }
 
+// POLY = false: the hard-wired heads (pde 0..6).  POLY = true: the polynomial residual head (pde 8, 9) in an instantiation of
+// its own, so the code of the hard-wired models does not change with it.
+template <bool POLY>
 __global__ void __launch_bounds__(THREADS, 2) fused_loss_grad(const Args p) {
   __shared__ double red[THREADS / 32];
   __shared__ int work_ctr;
@@ -401,7 +427,7 @@ __global__ void __launch_bounds__(THREADS, 2) fused_loss_grad(const Args p) {
   }
   __syncthreads();
   double part0 = 0.0, part1 = 0.0, part2 = 0.0, gl1 = 0.0, gl2 = 0.0;
-  if (p.pde >= 3) {
+  if (!POLY && p.pde >= 3) {
     const DiscArgs da{p.irk, p.tgt, p.n_d, p.n0p, p.dt, p.nu, p.kc, p.pde};
     const HeadSums hs = disc_head(da, npts, out, base, OUTV, SEED, A0, A1, l1, kap);
     part0 = hs.part0; part1 = hs.part1; gl1 = hs.gl1; gl2 = hs.gl2;
@@ -413,7 +439,49 @@ __global__ void __launch_bounds__(THREADS, 2) fused_loss_grad(const Args p) {
     double sd[4 * MAXOUT];
 #pragma unroll
     for (int c = 0; c < 4 * MAXOUT; c++) sd[c] = 0.0;
-    if (p.pde != 2) {
+    if (POLY) {
+      // polynomial residual (DESIGN 4.4d), BURGERS_INF / BURGERS_IDE loss structure: o = [u, u_x, u_t, u_xx]
+      const bool res = gp >= p.c0 && gp < p.c0 + p.n_c;
+      const double wf = res ? p.wf : 0.0;
+      const bool has_d = gp >= p.d0 && gp < p.d0 + p.n_d;
+      const double wd = has_d ? p.wd : 0.0;
+      const double r = has_d ? o[0] - __ldg(p.tgt + (gp - p.d0)) : 0.0;
+      const bool lam = p.pde == 9;                              // POLY_IDE: raw lambdas behind the net parameters
+      const double l1 = lam ? p.w[p.p_net] : 0.0, l2 = lam ? p.w[p.p_net + 1] : 0.0;
+      const double e1 = lam ? exp(l1) : 1.0, e2 = lam ? exp(l2) : 1.0;
+      double v[4], v2[4], v3[4];
+#pragma unroll
+      for (int j = 0; j < 4; j++) { v[j] = o[j]; v2[j] = v[j] * v[j]; v3[j] = v2[j] * v[j]; }
+      // f, df/dv_j = sum_k c_k kappa_k e_kj v_j^(e_kj - 1) prod_{i != j} v_i^e_ki, and df/d lambda_i (d e^l / dl = e^l)
+      double f = 0.0, d0 = 0.0, d1 = 0.0, d2 = 0.0, d3 = 0.0, f1 = 0.0, f2 = 0.0;
+      for (int k = 0; k < p.poly.n; k++) {
+        const int code = p.poly.code[k];
+        const int kind = code & 7, a0 = (code >> 3) & 3, a1 = (code >> 5) & 3, a2 = (code >> 7) & 3, a3 = (code >> 9) & 3;
+        const double q0 = pick_pow(v[0], v2[0], v3[0], a0), q1 = pick_pow(v[1], v2[1], v3[1], a1);
+        const double q2 = pick_pow(v[2], v2[2], v3[2], a2), q3 = pick_pow(v[3], v2[3], v3[3], a3);
+        const double q01 = q0 * q1, q23 = q2 * q3;
+        const double m = p.poly.coef[k] * (q01 * q23);
+        const double kv = kind == 0 ? 1.0 : (kind == 1 ? l1 : (kind == 2 ? l2 : (kind == 3 ? e1 : e2)));
+        const double ck = p.poly.coef[k] * kv;
+        f = fma(kv, m, f);
+        d0 = fma(ck * pick_dpow(v[0], v2[0], a0), q1 * q23, d0);
+        d1 = fma(ck * pick_dpow(v[1], v2[1], a1), q0 * q23, d1);
+        d2 = fma(ck * pick_dpow(v[2], v2[2], a2), q01 * q3, d2);
+        d3 = fma(ck * pick_dpow(v[3], v2[3], a3), q01 * q2, d3);
+        if (kind == 1 || kind == 3) f1 = fma(kind == 1 ? 1.0 : e1, m, f1);
+        else if (kind != 0) f2 = fma(kind == 2 ? 1.0 : e2, m, f2);
+      }
+      if (res && p.src) f -= __ldg(p.src + (gp - p.c0));
+      const double c = 2.0 * wf * f;
+      sd[0] = fma(c, d0, 2.0 * wd * r);
+      sd[1] = c * d1;
+      sd[2] = c * d2;
+      sd[3] = c * d3;
+      part0 = fma(wd * r, r, part0);
+      part2 = fma(wf * f, f, part2);
+      gl1 = fma(c, f1, gl1);
+      gl2 = fma(c, f2, gl2);
+    } else if (p.pde != 2) {
       // Burgers (inf_cont_burgers.py:59-90 / ide_cont_burgers.py:56-91): outputs o = [u, u_x, u_t, u_xx]
       const double u = o[0], ux = o[1], ut = o[2], uxx = o[3];
       const double wf = (gp >= p.c0 && gp < p.c0 + p.n_c) ? p.wf : 0.0;

@@ -148,6 +148,12 @@ struct pinn_handle {
   double* d_nsX = nullptr;                  // NS: training points [n][3] = (x, y, t); targets [n][2] in d_u
   long long nsx_cap = 0;
 
+  // POLY_INF / POLY_IDE: the residual's term table (n == 0: not set yet) and the source at the residual points (empty: 0)
+  pinn::generic::PolySpec poly{};
+  std::vector<double> h_src;
+  double* d_src = nullptr;
+  long long src_cap = 0;
+
   ncclComm_t comm = nullptr;
   // NVLink push exchange in the tail of every evaluation (optim_kernels.cuh: exchange_block)
   double* d_xchg = nullptr;            // [2][world][slot_len] doubles, then [2][world][n_blocks] u64 flags (IPC-exported)
@@ -163,6 +169,10 @@ namespace {
 // 1-D (x only) discrete-time models; identification: two snapshots, q outputs; inference: q+1 outputs
 bool is_disc(int pde) { return pde == PINN_BURGERS_DISC || pde == PINN_BURGERS_IDE_DISC || pde == PINN_KDV_IDE_DISC || pde == PINN_AC_DISC; }
 bool is_ide_disc(int pde) { return pde == PINN_BURGERS_IDE_DISC || pde == PINN_KDV_IDE_DISC; }
+// user-defined polynomial residual (pinn_set_residual) on the generic kernel's POLY instantiation
+bool is_poly(int pde) { return pde == PINN_POLY_INF || pde == PINN_POLY_IDE; }
+// continuous-time models whose data points are also the residual points
+bool residual_on_data(int pde) { return pde == PINN_BURGERS_IDE || pde == PINN_NS_IDE || pde == PINN_POLY_IDE; }
 
 bool is_burgers_net(const std::vector<int>& L) {
   if (L.size() != 10 || L[0] != 2 || L[9] != 1) return false;
@@ -460,7 +470,9 @@ int generic_launch_eval(pinn_t* h, const int* run_flag) {
   const bool idd = is_ide_disc(h->pde);
   const bool disc = is_disc(h->pde);
   if (disc && (!h->d_irk || h->irk_q + (idd ? 0 : 1) != h->layers.back())) return fail("discrete-time model: call pinn_set_irk first");
-  const bool nls = h->pde == PINN_NLS_INF, ide = h->pde == PINN_BURGERS_IDE;
+  const bool poly = is_poly(h->pde);
+  if (poly && h->poly.n == 0) return fail("polynomial residual model: call pinn_set_residual first (no residual is set)");
+  const bool nls = h->pde == PINN_NLS_INF, ide = h->pde == PINN_BURGERS_IDE || h->pde == PINN_POLY_IDE;
   const long long n_total = disc ? h->n_aux : (nls ? h->n_aux + h->n_c : (ide ? h->n_d : h->n_d + h->n_c));
   if (n_total <= 0) return fail("no points set (pinn_set_collocation / pinn_set_data)");
   const long long per = (n_total + h->n_cta - 1) / h->n_cta;
@@ -508,7 +520,13 @@ int generic_launch_eval(pinn_t* h, const int* run_flag) {
   static const bool generic_dfma = [] { const char* e = getenv("PINN_GENERIC_DFMA"); return e && e[0] == '1'; }();
   a.dmma = generic_dfma ? 0 : 1;
   a.partials = h->d_partials; a.pstride = h->pstride; a.run_flag = run_flag;
-  G::fused_loss_grad<<<grid, G::THREADS, 0, h->stream>>>(a);
+  if (poly) {
+    a.poly = h->poly;
+    a.src = h->h_src.empty() ? nullptr : h->d_src;
+    G::fused_loss_grad<true><<<grid, G::THREADS, 0, h->stream>>>(a);
+  } else {
+    G::fused_loss_grad<false><<<grid, G::THREADS, 0, h->stream>>>(a);
+  }
   CUDA_TRY(cudaGetLastError());
   h->launches++;
   pinn::ReduceMap map{};
@@ -736,9 +754,15 @@ int pinn_create(pinn_t** out, int pde_id, int n_layers, const int* layers, const
                 int device, int rank, int world, const void* nccl_uid) {
   if (!out || !layers || !lb || !ub) return fail("pinn_create: null argument");
   if (n_layers < 3 || n_layers > pinn::MAXL) return fail("pinn_create: need 3..16 layer sizes");
-  if (pde_id < 0 || pde_id > 7) return fail("pinn_create: unknown pde_id");
+  if (pde_id < 0 || pde_id > 9) return fail("pinn_create: unknown pde_id");
   const bool ns = pde_id == PINN_NS_IDE;
   if (ns && world > 1) return fail("pinn_create: the Navier-Stokes identification model runs on one GPU (world must be 1)");
+  if (is_poly(pde_id)) {
+    if (world > 1) return fail("pinn_create: the polynomial residual models run on one GPU (world must be 1)");
+    if (layers[0] != 2 || layers[n_layers - 1] != 1)
+      return fail("pinn_create: unknown pde_id for a [" + std::to_string(layers[0]) + ", ..., " + std::to_string(layers[n_layers - 1]) +
+                  "] net: the polynomial residual models (8, 9) take a net [2, ..., 1]: (x, t) -> u");
+  }
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
     return fail("pinn_create: no CUDA device -- this library has no CPU fallback");
@@ -780,12 +804,12 @@ int pinn_create(pinn_t** out, int pde_id, int n_layers, const int* layers, const
     // specialised DMMA kernels for the two BASELINE nets, generic DFMA kernel for any other layer list
     const char* fg = getenv("PINN_FORCE_GENERIC");
     const bool force = fg && fg[0] == '1';
-    const bool special = disc ? false : ((pde_id == PINN_NLS_INF) ? is_nls_net(h->layers) : is_burgers_net(h->layers));
+    const bool special = (disc || is_poly(pde_id)) ? false : ((pde_id == PINN_NLS_INF) ? is_nls_net(h->layers) : is_burgers_net(h->layers));
     h->kernel_kind = ns ? 3 : (special && !force) ? (pde_id == PINN_NLS_INF ? 1 : 0) : 2;
   }
   h->P_net = 0;
   for (int l = 0; l + 1 < n_layers; l++) h->P_net += layers[l] * layers[l + 1] + layers[l + 1];
-  h->P = h->P_net + ((pde_id == PINN_BURGERS_IDE || is_ide_disc(pde_id) || ns) ? 2 : 0);
+  h->P = h->P_net + ((pde_id == PINN_BURGERS_IDE || is_ide_disc(pde_id) || ns || pde_id == PINN_POLY_IDE) ? 2 : 0);
 
 #define CREATE_TRY(expr)                                                                          \
   do {                                                                                            \
@@ -874,7 +898,7 @@ int pinn_destroy(pinn_t* h) {
   if (h->d_xseq) cudaFree(h->d_xseq);
   if (h->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(h->comm);
   double* bufs[] = {h->d_w, h->d_R, h->d_partials, h->d_m, h->d_v, h->d_loss_ring, h->d_x, h->d_t, h->d_u, h->d_scrH, h->d_scrA, h->d_scrS, h->d_gH, h->d_gA, h->d_gS, h->d_irk, h->d_gold,
-                    h->d_d, h->d_S, h->d_Y, h->d_xfinal, h->d_fhist, h->d_px, h->d_pout, h->d_pscr, h->d_nsX};
+                    h->d_d, h->d_S, h->d_Y, h->d_xfinal, h->d_fhist, h->d_px, h->d_pout, h->d_pscr, h->d_nsX, h->d_src};
   for (double* b : bufs) if (b) cudaFree(b);
   if (h->d_step) cudaFree(h->d_step);
   if (h->d_lb) cudaFree(h->d_lb);
@@ -933,8 +957,9 @@ int pinn_get_params(pinn_t* h, double* p, int n) {
     p[0] = lam[0]; p[1] = std::exp(lam[1]);         // ide_cont_burgers.py:109-114, ide_disc_burgers.py:138-143
     return 0;
   }
-  if (h->pde == PINN_NS_IDE) {
-    if (n != 2) return fail("pinn_get_params: NS_IDE has two parameters (lambda_1, lambda_2)");
+  if (h->pde == PINN_NS_IDE || h->pde == PINN_POLY_IDE) {
+    if (n != 2) return fail(h->pde == PINN_NS_IDE ? "pinn_get_params: NS_IDE has two parameters (lambda_1, lambda_2)"
+                                                  : "pinn_get_params: POLY_IDE has two parameters (the raw lambda_1, lambda_2)");
     CUDA_TRY(cudaSetDevice(h->device));
     CUDA_TRY(cudaMemcpyAsync(p, h->d_w + h->P_net, 16, cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(cudaStreamSynchronize(h->stream));
@@ -972,7 +997,7 @@ int pinn_set_irk(pinn_t* h, const double* irk, int q) {
 
 int pinn_set_collocation(pinn_t* h, const double* x, const double* t, int64_t n, int64_t n_global) {
   if (!h) return fail("null handle");
-  if (h->pde == PINN_BURGERS_IDE || h->pde == PINN_NS_IDE)
+  if (residual_on_data(h->pde))
     return fail("pinn_set_collocation: identification uses the data points as residual points");
   if (is_disc(h->pde))
     return fail("pinn_set_collocation: the discrete-time models have no collocation set (snapshot / boundary points only)");
@@ -988,6 +1013,7 @@ int pinn_set_collocation(pinn_t* h, const double* x, const double* t, int64_t n,
   }
   h->n_c = n; h->n_c_global = n_global;
   h->map_x = h->map_t = nullptr;
+  h->h_src.clear();                               // POLY_INF: new residual points, the source is 0 until set again
   return 0;
 }
 
@@ -1072,6 +1098,54 @@ int pinn_set_data(pinn_t* h, const double* X, int64_t n, int in_dim, const doubl
     CUDA_TRY(cudaStreamSynchronize(h->stream));
   }
   h->n_d = n; h->n_aux = n; h->d_out_dim = out_dim; h->data_weight = weight;
+  if (h->pde == PINN_POLY_IDE) h->h_src.clear();  // new residual points: the source is 0 until set again
+  return 0;
+}
+
+int pinn_set_residual(pinn_t* h, int n_terms, const double* coef, const int* kind, const int* exps) {
+  if (!h) return fail("null handle");
+  if (!is_poly(h->pde)) return fail("pinn_set_residual: only the polynomial residual models (POLY_INF, POLY_IDE) take a residual spec");
+  if (n_terms < 1 || n_terms > pinn::generic::POLY_MAXT)
+    return fail("pinn_set_residual: n_terms = " + std::to_string(n_terms) + " is outside 1..16");
+  if (!coef || !kind || !exps) return fail("pinn_set_residual: null argument");
+  pinn::generic::PolySpec s{};
+  s.n = n_terms;
+  for (int k = 0; k < n_terms; k++) {
+    const std::string term = "pinn_set_residual: term " + std::to_string(k) + ": ";
+    if (!std::isfinite(coef[k])) return fail(term + "the coefficient is not finite");
+    if (kind[k] < 0 || kind[k] > 4) return fail(term + "kind " + std::to_string(kind[k]) + " is outside 0..4 (1, l1, l2, e^l1, e^l2)");
+    if (kind[k] != 0 && h->pde == PINN_POLY_INF)
+      return fail(term + "POLY_INF has no trainable lambdas: every kind must be 0 (use POLY_IDE for l1, l2, e^l1, e^l2)");
+    int code = kind[k], any = 0;
+    for (int j = 0; j < 4; j++) {
+      const int e = exps[4 * k + j];
+      if (e < 0 || e > 3) return fail(term + "exponent " + std::to_string(e) + " of stream " + std::to_string(j) + " is outside 0..3");
+      code |= e << (3 + 2 * j);
+      any |= e;
+    }
+    if (!any) return fail(term + "all four exponents are 0 (a constant term belongs in the source)");
+    s.code[k] = code;
+    s.coef[k] = coef[k];
+  }
+  h->poly = s;
+  return 0;
+}
+
+int pinn_set_source(pinn_t* h, const double* src, int64_t n) {
+  if (!h) return fail("null handle");
+  if (!is_poly(h->pde)) return fail("pinn_set_source: only the polynomial residual models (POLY_INF, POLY_IDE) take a source");
+  const int64_t want = pinn_num_residual_points(h);
+  if (n != want)
+    return fail("pinn_set_source: " + std::to_string(n) + " values given but " + std::to_string(want) +
+                " residual points are stored (pinn_num_residual_points)");
+  if (n > 0 && !src) return fail("pinn_set_source: null argument");
+  CUDA_TRY(cudaSetDevice(h->device));
+  if (n > 0) {
+    if (ensure(&h->d_src, &h->src_cap, n)) return -1;
+    CUDA_TRY(cudaMemcpyAsync(h->d_src, src, n * 8, cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(cudaStreamSynchronize(h->stream));
+  }
+  h->h_src.assign(src, src + n);
   return 0;
 }
 
@@ -1357,7 +1431,7 @@ int pinn_derivatives(pinn_t* h, const double* X, int64_t n, double* out) {
 int64_t pinn_num_residual_points(const pinn_t* h) {
   if (!h) return -1;
   if (is_disc(h->pde)) return 0;
-  return (h->pde == PINN_BURGERS_IDE || h->pde == PINN_NS_IDE) ? h->n_d : h->n_c;
+  return residual_on_data(h->pde) ? h->n_d : h->n_c;
 }
 
 int pinn_residual(pinn_t* h, double* f_out, int64_t n_rows) {
@@ -1371,7 +1445,8 @@ int pinn_residual(pinn_t* h, double* f_out, int64_t n_rows) {
     CUDA_TRY(cudaSetDevice(h->device));
     return ns_probe(h, h->d_nsX, h->n_d, 2, f_out);
   }
-  const bool ide = h->pde == PINN_BURGERS_IDE;
+  const bool ide = h->pde == PINN_BURGERS_IDE || h->pde == PINN_POLY_IDE;
+  if (is_poly(h->pde) && h->poly.n == 0) return fail("pinn_residual: call pinn_set_residual first (no residual is set)");
   const int64_t n = ide ? h->n_d : h->n_c;
   if (n_rows != n)
     return fail("pinn_residual: the output buffer holds " + std::to_string(n_rows) + " rows but " + std::to_string(n) +
@@ -1389,6 +1464,25 @@ int pinn_residual(pinn_t* h, double* f_out, int64_t n_rows) {
       const double h2 = u * u + v * v;
       f_out[2 * i] = ut + 0.5 * vxx + h2 * v;
       f_out[2 * i + 1] = vt - 0.5 * uxx - h2 * u;
+    }
+    return 0;
+  }
+  if (is_poly(h->pde)) {
+    // the kernel head's f, term by term on the host: sum_k c_k kappa_k prod_j v_j^e_kj - s
+    double lam[2] = {0.0, 0.0};
+    if (ide) CUDA_TRY(cudaMemcpy(lam, h->d_w + h->P_net, 16, cudaMemcpyDeviceToHost));
+    const double kv[5] = {1.0, lam[0], lam[1], std::exp(lam[0]), std::exp(lam[1])};
+    for (int64_t i = 0; i < n; i++) {
+      const double* d = &D[i * 4];
+      double f = 0.0;
+      for (int k = 0; k < h->poly.n; k++) {
+        const int code = h->poly.code[k];
+        double m = h->poly.coef[k];
+        for (int j = 0; j < 4; j++)
+          for (int e = (code >> (3 + 2 * j)) & 3; e > 0; e--) m *= d[j];
+        f += kv[code & 7] * m;
+      }
+      f_out[i] = h->h_src.empty() ? f : f - h->h_src[i];
     }
     return 0;
   }
@@ -1492,7 +1586,8 @@ int pinn_kernel_info(pinn_t* h, char* buf, int buflen) {
     CUDA_TRY(cudaFuncGetAttributes(&fa, pinn::nsid::fused_loss_grad));
     smem = 0; threads = pinn::nsid::THREADS;
   } else if (h->kernel_kind == 2) {
-    CUDA_TRY(cudaFuncGetAttributes(&fa, pinn::generic::fused_loss_grad));
+    if (is_poly(h->pde)) CUDA_TRY(cudaFuncGetAttributes(&fa, pinn::generic::fused_loss_grad<true>));
+    else CUDA_TRY(cudaFuncGetAttributes(&fa, pinn::generic::fused_loss_grad<false>));
     smem = 0; threads = pinn::generic::THREADS;
   } else if (h->pde == PINN_NLS_INF) {
     CUDA_TRY(cudaFuncGetAttributes(&fa, pinn::nls::fused_loss_grad));

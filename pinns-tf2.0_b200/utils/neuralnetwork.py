@@ -10,6 +10,7 @@ definitions load unchanged.  Everything is float64, as in the reference (:24-26)
 import numpy as np
 
 import pinn_cabi
+import poly_spec
 from custom_lbfgs import Struct, lbfgs
 
 
@@ -91,7 +92,10 @@ _NATIVE_OVERRIDES = {}
 
 class NeuralNetwork(object):
     pde = None           # optional explicit PDE id: "burgers_inf" | "burgers_ide" | "nls_inf" | "burgers_disc" | "burgers_ide_disc"
-    #                      | "kdv_ide_disc" | "ac_disc" | "ns_ide" (the last three are never guessed from attributes)
+    #                      | "kdv_ide_disc" | "ac_disc" | "ns_ide" | "poly" (the last four are never guessed from attributes)
+    residual = None      # pde = "poly": the residual as a string, e.g. "u_t + u*u_x - nu*u_xx" (utils/poly_spec.py); a spec that
+    #                      mentions l1 / l2 is identification (fit(X_u, u), residual on the data points), otherwise inference
+    #                      (collocation x_f, t_f).  An optional method source(x, t) gives s in f = ... - s.
     weight_seed = 1234   # stands in for tf.random.set_seed(1234) (inf_cont_burgers.py:10)
 
     def __init_subclass__(cls, **kw):
@@ -159,9 +163,37 @@ class NeuralNetwork(object):
                 tag = "burgers_inf"
             else:
                 raise pinn_cabi.PinnError("cannot recognise the PDE of %s: set the class attribute `pde`" % type(self).__name__)
+        if tag == "poly":
+            return pinn_cabi.POLY_IDE if self._poly_spec().identification else pinn_cabi.POLY_INF
         return {"burgers_inf": pinn_cabi.BURGERS_INF, "burgers_ide": pinn_cabi.BURGERS_IDE, "nls_inf": pinn_cabi.NLS_INF,
                 "burgers_disc": pinn_cabi.BURGERS_DISC, "burgers_ide_disc": pinn_cabi.BURGERS_IDE_DISC,
                 "kdv_ide_disc": pinn_cabi.KDV_IDE_DISC, "ac_disc": pinn_cabi.AC_DISC, "ns_ide": pinn_cabi.NS_IDE}[tag]
+
+    def _poly_spec(self):
+        """The parsed `residual` string (pde = "poly"); free names resolve to numeric attributes of the instance."""
+        if getattr(self, "_poly_cache", None) is None:
+            def resolve(name):
+                v = getattr(self, name, None)
+                if isinstance(v, (bool, np.bool_, str, bytes)) or v is None or callable(v):
+                    return None
+                try:
+                    a = np.asarray(v, dtype=np.float64)
+                except (TypeError, ValueError):
+                    return None
+                return float(a.reshape(-1)[0]) if a.size == 1 else None
+            try:
+                self._poly_cache = poly_spec.parse(self.residual, resolve)
+            except poly_spec.SpecError as e:
+                raise pinn_cabi.PinnError("%s.residual: %s" % (type(self).__name__, e))
+        return self._poly_cache
+
+    def _upload_source(self, X, h=None):
+        """pde = "poly": source(x, t) on the residual points X (N, 2) just bound, when the subclass defines it."""
+        fn = getattr(self, "source", None)
+        if callable(fn):
+            X = np.asarray(X, dtype=np.float64)
+            s = np.asarray(fn(X[:, 0:1], X[:, 1:2]), dtype=np.float64)
+            (h or self._native()).set_source(np.broadcast_to(s.reshape(-1) if s.size == X.shape[0] else s, (X.shape[0],)))
 
     def _two_snapshots(self):
         return self._pde_id() in _TWO_SNAPSHOT
@@ -190,6 +222,15 @@ class NeuralNetwork(object):
                 h.set_irk(np.asarray(self.IRK_weights, dtype=np.float64))
             elif pde == pinn_cabi.NS_IDE:                            # NavierStokes.py: raw lambdas, both 0.0 unless the class sets them
                 w = np.concatenate([w, [_scalar(getattr(self, "lambda_1", 0.0)), _scalar(getattr(self, "lambda_2", 0.0))]])
+            elif pde in _POLY:                                       # utils/poly_spec.py
+                h.set_residual(self._poly_spec().terms)
+                if pde == pinn_cabi.POLY_IDE:                        # raw lambdas, 0.0 unless the class sets them
+                    w = np.concatenate([w, [_scalar(getattr(self, "lambda_1", 0.0)), _scalar(getattr(self, "lambda_2", 0.0))]])
+                else:
+                    X_f = np.hstack([np.asarray(self.x_f, dtype=np.float64).reshape(-1, 1),
+                                     np.asarray(self.t_f, dtype=np.float64).reshape(-1, 1)])
+                    h.set_collocation(X_f[:, 0], X_f[:, 1], getattr(self, "n_f_global", None))
+                    self._upload_source(X_f, h)
             elif pde == pinn_cabi.BURGERS_IDE:
                 l1 = float(np.asarray(self.lambda_1.numpy() if hasattr(self.lambda_1, "numpy") else self.lambda_1).reshape(-1)[0])
                 l2 = float(np.asarray(self.lambda_2.numpy() if hasattr(self.lambda_2, "numpy") else self.lambda_2).reshape(-1)[0])
@@ -221,6 +262,8 @@ class NeuralNetwork(object):
         if self._bound != key:
             Xa, ua = np.asarray(X, dtype=np.float64), np.asarray(u, dtype=np.float64)
             self._native().set_data(Xa, ua, getattr(self, "data_weight", 1.0))
+            if self._pde_id() == pinn_cabi.POLY_IDE:         # the data points are the residual points
+                self._upload_source(Xa)
             self._bound = key
             self._bound_refs = (X, u)
 
@@ -350,7 +393,9 @@ class NeuralNetwork(object):
 # two-snapshot discrete-time identification models: fit(x_0, u_0, x_1, u_1), predict -> (U_0, U_1), flat vector ends with l1, l2
 _TWO_SNAPSHOT = (pinn_cabi.BURGERS_IDE_DISC, pinn_cabi.KDV_IDE_DISC)
 # every model whose flat vector ends with [lambda_1, lambda_2]
-_LAMBDAS = (pinn_cabi.BURGERS_IDE, pinn_cabi.NS_IDE) + _TWO_SNAPSHOT
+_LAMBDAS = (pinn_cabi.BURGERS_IDE, pinn_cabi.NS_IDE, pinn_cabi.POLY_IDE) + _TWO_SNAPSHOT
+# user-defined polynomial residuals (pde = "poly")
+_POLY = (pinn_cabi.POLY_INF, pinn_cabi.POLY_IDE)
 
 
 def _scalar(v):
@@ -383,6 +428,19 @@ def _native_f_model(self, *args):
     """f_model (inf_cont_burgers.py:65-90 / ide_cont_burgers.py:56-85 / inf_cont_schrodinger.py:79-105): on the stored
     residual points, or -- identification, where the reference passes the points explicitly -- on the given points."""
     n = self._native()
+    if self._pde_id() in _POLY:
+        if args:                                          # on the given points: streams from the device, the spec on the host
+            X = np.asarray(args[0], dtype=np.float64)
+            U, Ux, Ut, Uxx = n.derivatives(X)
+            lam = n.get_weights()[-2:] if n.pde == pinn_cabi.POLY_IDE else (0.0, 0.0)
+            f = poly_spec.evaluate(self._poly_spec().terms, (U, Ux, Ut, Uxx), *lam)
+            fn = getattr(self, "source", None)
+            if callable(fn):
+                f = f - np.asarray(fn(X[:, 0:1], X[:, 1:2]), dtype=np.float64).reshape(f.shape)
+            return _t(f)
+        if n.pde == pinn_cabi.POLY_IDE and self._bound is None:
+            raise pinn_cabi.PinnError("f_model(): no data points are bound yet -- call fit()/grad() first, or pass the points")
+        return _t(n.residual())
     if self._pde_id() == pinn_cabi.NS_IDE and args:
         return _ns_fields(self, args[0])[3:]
     if self._pde_id() == pinn_cabi.BURGERS_IDE:
@@ -506,8 +564,8 @@ def _native_get_params(self, numpy=False):
     pde = self._pde_id()
     if pde == pinn_cabi.BURGERS_INF:
         return self.nu
-    if pde == pinn_cabi.NS_IDE:
-        l1, l2 = self._native().get_weights()[-2:]     # raw lambdas (NavierStokes.py)
+    if pde in (pinn_cabi.NS_IDE, pinn_cabi.POLY_IDE):
+        l1, l2 = self._native().get_weights()[-2:]     # raw lambdas (NavierStokes.py; the poly residual's l1, l2)
         return (l1, l2) if numpy else (_t([l1]), _t([l2]))
     if pde in (pinn_cabi.BURGERS_IDE,) + _TWO_SNAPSHOT:
         w = self._native().get_weights()

@@ -14,6 +14,10 @@ _HERE = os.path.dirname(os.path.realpath(__file__))
 LIB_PATH = os.environ.get("PINN_LIB") or os.path.join(_HERE, "..", "lib", "libpinn_b200.so")
 
 BURGERS_INF, BURGERS_IDE, NLS_INF, BURGERS_DISC, BURGERS_IDE_DISC, KDV_IDE_DISC, AC_DISC, NS_IDE = 0, 1, 2, 3, 4, 5, 6, 7
+# user-defined polynomial residual (Pinn.set_residual) with the loss structure of BURGERS_INF / BURGERS_IDE
+POLY_INF, POLY_IDE = 8, 9
+# kappa_k of a polynomial residual term, in the order of pinn_set_residual's kind
+POLY_KINDS = ("1", "l1", "l2", "exp(l1)", "exp(l2)")
 # Navier-Stokes derivative streams, in the order of pinn_derivatives' blocks
 NS_STREAMS = ("u", "x", "y", "t", "xx", "xy", "yy", "xt", "yt", "xxx", "xxy", "xyy", "yyy")
 LBFGS_REASONS = {0: "running", 1: "max iterations", 2: "max evaluations", 3: "optimality", 4: "step below tolX",
@@ -42,6 +46,8 @@ SIGNATURES = {
     "pinn_set_data": (C.c_int, [C.c_void_p, _dp, C.c_int64, C.c_int, _dp, C.c_int, C.c_double]),
     "pinn_set_snapshot": (C.c_int, [C.c_void_p, C.c_int, _dp, C.c_int64, _dp]),
     "pinn_set_boundary": (C.c_int, [C.c_void_p, _dp, C.c_int64]),
+    "pinn_set_residual": (C.c_int, [C.c_void_p, C.c_int, _dp, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "pinn_set_source": (C.c_int, [C.c_void_p, _dp, C.c_int64]),
     "pinn_set_weights": (C.c_int, [C.c_void_p, _dp, C.c_int64]),
     "pinn_get_weights": (C.c_int, [C.c_void_p, _dp, C.c_int64]),
     "pinn_loss_grad": (C.c_int, [C.c_void_p, _dp, _dp, _dp, _dp]),
@@ -165,7 +171,7 @@ class Pinn(object):
 
     def get_params(self):
         n = {BURGERS_INF: 1, BURGERS_IDE: 2, NLS_INF: 0, BURGERS_DISC: 2, BURGERS_IDE_DISC: 2, KDV_IDE_DISC: 2, AC_DISC: 3,
-             NS_IDE: 2}[self.pde]
+             NS_IDE: 2, POLY_INF: 0, POLY_IDE: 2}[self.pde]
         out = np.zeros(max(n, 1))
         self._ck(self.lib.pinn_get_params(self.h, _p(out), n))
         return out[:n]
@@ -206,6 +212,23 @@ class Pinn(object):
     def set_boundary(self, tb):
         tb = _arr(tb).reshape(-1)
         self._ck(self.lib.pinn_set_boundary(self.h, _p(tb), tb.size))
+
+    def set_residual(self, terms):
+        """POLY_INF / POLY_IDE: terms = [(coef, kind, (e_u, e_ux, e_ut, e_uxx)), ...], 1 to 16 of them; kind 0..4 selects
+        kappa = 1, l1, l2, exp(l1), exp(l2) (POLY_KINDS)."""
+        terms = list(terms)
+        n = len(terms)
+        coef = _arr([float(c) for c, _, _ in terms] or [0.0])
+        kind = (C.c_int * max(n, 1))(*[int(k) for _, k, _ in terms])
+        exps = (C.c_int * max(4 * n, 1))(*[int(e) for _, _, es in terms for e in es])
+        if any(len(es) != 4 for _, _, es in terms):
+            raise PinnError("set_residual: each term needs four exponents (u, u_x, u_t, u_xx)")
+        self._ck(self.lib.pinn_set_residual(self.h, n, _p(coef), kind, exps))
+
+    def set_source(self, s):
+        """POLY_INF / POLY_IDE: the source s at the stored residual points (reset to 0 whenever new residual points are set)."""
+        s = _arr(s).reshape(-1)
+        self._ck(self.lib.pinn_set_source(self.h, _p(s), s.size))
 
     # ---- parameters
     def set_weights(self, w):
