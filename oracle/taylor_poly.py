@@ -23,13 +23,16 @@ def _pw(v, e):
     return out
 
 
-def poly_terms(terms, V, l1=0.0, l2=0.0, dtype=np.float64):
-    """(f without the source, [df/dv_j for j = u, u_x, u_t, u_xx], df/dl1, df/dl2) on the stream arrays V."""
+def poly_terms(terms, V, l1=0.0, l2=0.0, dtype=np.float64, magnitudes=False):
+    """(f without the source, [df/dv_j for j = u, u_x, u_t, u_xx], df/dl1, df/dl2) on the stream arrays V.
+    magnitudes=True appends the term-wise magnitudes of df/dl1 and df/dl2 (sum_k |d kappa_k/dl_i m_k|): the scale of the
+    rounding of a sum over the terms, which |df/dl_i| under-counts where terms cancel (Fisher-KPP's -l1 u + l1 u^2 at u = 1)."""
     e1, e2 = np.exp(dtype(l1)), np.exp(dtype(l2))
     kv = (dtype(1), dtype(l1), dtype(l2), e1, e2)
     f = np.zeros_like(V[0])
     D = [np.zeros_like(V[0]) for _ in range(4)]
     f1, f2 = np.zeros_like(V[0]), np.zeros_like(V[0])
+    a1, a2 = np.zeros_like(V[0]), np.zeros_like(V[0])
     for c, k, e in terms:
         c = dtype(c)
         q = [_pw(V[j], e[j]) for j in range(4)]
@@ -44,9 +47,11 @@ def poly_terms(terms, V, l1=0.0, l2=0.0, dtype=np.float64):
                 D[j] = D[j] + c * kv[k] * e[j] * _pw(V[j], e[j] - 1) * other
         if k in (1, 3):
             f1 = f1 + (m if k == 1 else e1 * m)
+            a1 = a1 + np.abs(m if k == 1 else e1 * m)
         elif k in (2, 4):
             f2 = f2 + (m if k == 2 else e2 * m)
-    return f, D, f1, f2
+            a2 = a2 + np.abs(m if k == 2 else e2 * m)
+    return (f, D, f1, f2) + ((a1, a2) if magnitudes else ())
 
 
 def poly_loss_grad(w, layers, lb, ub, terms, X_u, u, X_f=None, source=None, identification=False, n_f_global=None,
@@ -63,7 +68,7 @@ def poly_loss_grad(w, layers, lb, ub, terms, X_u, u, X_f=None, source=None, iden
         wn, l1, l2 = w, dtype(0), dtype(0)
     nf = X_f.shape[0] if identification else (n_f_global or X_f.shape[0])
     (U, Ux, Ut, Uxx), st = forward(wn, layers, lb, ub, X_f, dtype)
-    f, D, f1, f2 = poly_terms(terms, (U, Ux, Ut, Uxx), l1, l2, dtype)
+    f, D, f1, f2, *a = poly_terms(terms, (U, Ux, Ut, Uxx), l1, l2, dtype, magnitudes)
     if source is not None:
         f = f - np.asarray(source, dtype=dtype).reshape(-1, 1)
     c = 2.0 * f / nf
@@ -80,7 +85,7 @@ def poly_loss_grad(w, layers, lb, ub, terms, X_u, u, X_f=None, source=None, iden
     if identification:
         g = np.concatenate([g, [np.sum(c * f1), np.sum(c * f2)]])
         if magnitudes:
-            m = np.concatenate([m, [np.sum(np.abs(c * f1)), np.sum(np.abs(c * f2))]])
+            m = np.concatenate([m, [np.sum(np.abs(c) * a[0]), np.sum(np.abs(c) * a[1])]])
     return (mse_u + mse_f, g, (mse_u, mse_f)) + ((m,) if magnitudes else ())
 
 

@@ -14,6 +14,11 @@ the input scale factor 2/(ub0 - lb0) is exactly 1) and with nu = 0.01/pi (which 
   from 0.25x to 8x the initialisation scale.
 
 Each test prints the worst ||g_B - g*_B|| / bound it saw (run with -s to read them).
+
+Held per block here: the specialised Burgers kernels (v2, v1), the Schrodinger kernel, the generic kernel's continuous-time
+Burgers heads and its discrete-time Burgers heads (pde 3, 4).  tests/test_gpu_precision_heads.py holds the generic kernel's
+KdV (pde 5), Allen-Cahn (pde 6) and polynomial residual (pde 8, 9) heads to the same rule with these helpers, and
+tests/test_gpu_ns.py the Navier-Stokes kernel.
 """
 import json
 import os
