@@ -142,8 +142,8 @@ def test_probes_residual_and_predict(cabi):
     assert rel(p.predict(g["X_probe"]), g["probe"][:, 0]) <= 1e-11
     f = p.residual()
     assert f.shape == g["residual"].shape and rel(f, g["residual"]) <= 1e-10
-    # a wide net takes the chunked probe
-    layers, lb, ub, X, uv, w = ns_inputs([256, 256], 700, 5)
+    # a width-256 net probes in chunks of 5 041 points: 11 000 points take two full chunks and a ragged third
+    layers, lb, ub, X, uv, w = ns_inputs([256, 256], 11000, 5)
     q = make(cabi, layers, lb, ub, X, uv)
     q.set_weights(w)
     O, _ = tn.forward_ns(w[:-2], layers, lb, ub, X)

@@ -18,7 +18,9 @@ Each test prints the worst ||g_B - g*_B|| / bound it saw (run with -s to read th
 Held per block here: the specialised Burgers kernels (v2, v1), the Schrodinger kernel, the generic kernel's continuous-time
 Burgers heads and its discrete-time Burgers heads (pde 3, 4).  tests/test_gpu_precision_heads.py holds the generic kernel's
 KdV (pde 5), Allen-Cahn (pde 6) and polynomial residual (pde 8, 9) heads to the same rule with these helpers, and
-tests/test_gpu_ns.py the Navier-Stokes kernel.
+tests/test_gpu_ns.py the Navier-Stokes kernel.  tests/test_gpu_precision_load.py holds the specialised Burgers and Schrodinger
+kernels, the generic kernel's Burgers and Schrodinger heads, the Navier-Stokes kernel and the probes at the per-CTA loads they
+run at (up to 2M points), on shuffled copies of a base set.
 """
 import json
 import os
