@@ -114,6 +114,8 @@ int pinn_get_params(pinn_t* h, double* p, int n);
 /* KDV_IDE_DISC takes the BURGERS_IDE_DISC layout, AC_DISC the BURGERS_DISC one. */
 int pinn_set_irk(pinn_t* h, const double* irk, int q);
 
+/* Point, target and weight inputs are not checked for finiteness: NaN and +-Inf propagate as in the reference (DESIGN §1,
+ * "Non-finite values"). */
 /* Collocation points of THIS rank: x_f, t_f (inf_cont_burgers.py:55-56; inf_cont_schrodinger.py:56-57).
  * n_global = N_f over all ranks (the MSE_f denominator); pass n when world == 1. */
 int pinn_set_collocation(pinn_t* h, const double* x, const double* t, int64_t n, int64_t n_global);

@@ -319,7 +319,8 @@ __global__ void __launch_bounds__(THREADS, 1) fused_loss_grad(const Args p) {
     const bool in_set = pt < p.n_total;
     const long long pc = in_set ? pt : p.n_total - 1;
     const double xr = __ldg(p.x + pc), tr = __ldg(p.t + pc);
-    const double wf = (in_set && pt >= p.c0 && pt < p.c0 + p.n_c) ? p.wf : 0.0;
+    const bool in_c = in_set && pt >= p.c0 && pt < p.c0 + p.n_c;
+    const double wf = in_c ? p.wf : 0.0;
     const bool has_d = in_set && pt >= p.d0 && pt < p.d0 + p.n_d;
     const double wd = has_d ? p.wd : 0.0;
     const double ut = has_d ? __ldg(p.utgt + (pt - p.d0)) : 0.0;
@@ -386,14 +387,15 @@ __global__ void __launch_bounds__(THREADS, 1) fused_loss_grad(const Args p) {
     double seed[4];
     {
       const double u = out[0], ux = out[1], utt = out[2], uxx = out[3];
-      const double f = utt + l1 * u * ux - kap * uxx;        // inf_cont_burgers.py:90 / ide_cont_burgers.py:85
-      const double r = u - ut;
+      // f and r are selected, not weighted by 0, outside their sets: 0 * NaN or 0 * Inf would reach the other set's part
+      const double f = in_c ? utt + l1 * u * ux - kap * uxx : 0.0;   // inf_cont_burgers.py:90 / ide_cont_burgers.py:85
+      const double r = has_d ? u - ut : 0.0;
       const double c = 2.0 * wf * f;
       seed[0] = fma(c * l1, ux, 2.0 * wd * r);
       seed[1] = c * l1 * u;
       seed[2] = c;
       seed[3] = -c * kap;
-      if (q == 0) {
+      if (q == 0 && in_set) {                                // a padded lane (clamped copy of the last point) adds nothing
         loss_d = fma(wd * r, r, loss_d);
         loss_f = fma(wf * f, f, loss_f);
         gl1 = fma(c * u, ux, gl1);

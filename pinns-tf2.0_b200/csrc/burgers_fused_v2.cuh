@@ -438,7 +438,8 @@ __global__ void __maxnreg__(252) fused_loss_grad(const Args p) {
       const bool in_set = pt < p.n_total;
       const double xr = xr_next, tr = tr_next;
       if (it + 1 < n_tiles) load_xt(it + 1, xr_next, tr_next);
-      const double wf = (in_set && pt >= p.c0 && pt < p.c0 + p.n_c) ? p.wf : 0.0;
+      const bool in_c = in_set && pt >= p.c0 && pt < p.c0 + p.n_c;
+      const double wf = in_c ? p.wf : 0.0;
       const bool has_d = in_set && pt >= p.d0 && pt < p.d0 + p.n_d;
       const double wd = has_d ? p.wd : 0.0;
       const double ut = has_d ? __ldg(p.utgt + (pt - p.d0)) : 0.0;
@@ -502,15 +503,16 @@ __global__ void __maxnreg__(252) fused_loss_grad(const Args p) {
         }
         out[0] += Wsm[boff(8)];
         const double u = out[0], ux = out[1], utt = out[2], uxx = out[3];
-        const double f = utt + l1 * u * ux - kap * uxx;      // inf_cont_burgers.py:90 / ide_cont_burgers.py:85
-        const double r = u - ut;
+        // f and r are selected, not weighted by 0, outside their sets: 0 * NaN or 0 * Inf would reach the other set's part
+        const double f = in_c ? utt + l1 * u * ux - kap * uxx : 0.0;   // inf_cont_burgers.py:90 / ide_cont_burgers.py:85
+        const double r = has_d ? u - ut : 0.0;
         const double cc = 2.0 * wf * f;
         double seed[4];
         seed[0] = fma(cc * l1, ux, 2.0 * wd * r);
         seed[1] = cc * l1 * u;
         seed[2] = cc;
         seed[3] = -cc * kap;
-        if (q == 0) {
+        if (q == 0 && in_set) {                              // a padded lane (clamped copy of the last point) adds nothing
           loss_d = fma(wd * r, r, loss_d);
           loss_f = fma(wf * f, f, loss_f);
           gl1 = fma(cc * u, ux, gl1);

@@ -472,6 +472,7 @@ __global__ void __launch_bounds__(THREADS, 2) fused_loss_grad(const Args p) {
         else if (kind != 0) f2 = fma(kind == 2 ? 1.0 : e2, m, f2);
       }
       if (res && p.src) f -= __ldg(p.src + (gp - p.c0));
+      f = res ? f : 0.0;                                        // selected, not weighted by 0: see the Burgers head
       const double c = 2.0 * wf * f;
       sd[0] = fma(c, d0, 2.0 * wd * r);
       sd[1] = c * d1;
@@ -484,11 +485,13 @@ __global__ void __launch_bounds__(THREADS, 2) fused_loss_grad(const Args p) {
     } else if (p.pde != 2) {
       // Burgers (inf_cont_burgers.py:59-90 / ide_cont_burgers.py:56-91): outputs o = [u, u_x, u_t, u_xx]
       const double u = o[0], ux = o[1], ut = o[2], uxx = o[3];
-      const double wf = (gp >= p.c0 && gp < p.c0 + p.n_c) ? p.wf : 0.0;
+      const bool res = gp >= p.c0 && gp < p.c0 + p.n_c;
+      const double wf = res ? p.wf : 0.0;
       const bool has_d = gp >= p.d0 && gp < p.d0 + p.n_d;
       const double wd = has_d ? p.wd : 0.0;
       const double r = has_d ? u - __ldg(p.tgt + (gp - p.d0)) : 0.0;
-      const double f = ut + l1 * u * ux - kap * uxx;
+      // f is selected, not weighted by 0, off the residual set: 0 * NaN or 0 * Inf would reach the data part
+      const double f = res ? ut + l1 * u * ux - kap * uxx : 0.0;
       const double c = 2.0 * wf * f;
       sd[0] = fma(c * l1, ux, 2.0 * wd * r);
       sd[1] = c * l1 * u;

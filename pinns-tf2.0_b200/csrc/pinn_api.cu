@@ -609,7 +609,7 @@ int ns_probe(pinn_t* h, const double* dX, int64_t n, int mode, double* out_host)
 }
 
 // NLS: (re)assemble the auxiliary block [initial-condition points | pad to even | (lb_k, ub_k) pairs] right-aligned in
-// the data region (inf_cont_schrodinger.py:50-53 builds X_lb=(lb0,tb), X_ub=(ub0,tb)).
+// the data region (inf_cont_schrodinger.py:50-53 builds X_lb=(0*tb+lb0,tb), X_ub=(0*tb+ub0,tb)).
 int nls_upload_points(pinn_t* h) {
   const long long n0 = h->n_d, n0p = (n0 + 1) & ~1LL, nb = h->n_b;
   const long long n_aux = n0p + 2 * nb;
@@ -619,8 +619,9 @@ int nls_upload_points(pinn_t* h) {
   for (long long i = 0; i < n0; i++) { h->stage_x[i] = h->h_icx[i]; h->stage_t[i] = h->h_ict[i]; }
   if (n0p > n0) { h->stage_x[n0] = h->lb[0]; h->stage_t[n0] = h->lb[1]; }     // inert alignment point
   for (long long k = 0; k < nb; k++) {
-    h->stage_x[n0p + 2 * k] = h->lb[0];     h->stage_t[n0p + 2 * k] = h->h_tb[k];
-    h->stage_x[n0p + 2 * k + 1] = h->ub[0]; h->stage_t[n0p + 2 * k + 1] = h->h_tb[k];
+    // x as the reference forms it, 0 * tb + lb0: NaN for an infinite or NaN tb, lb0 (ub0) for every finite one
+    h->stage_x[n0p + 2 * k] = 0.0 * h->h_tb[k] + h->lb[0];     h->stage_t[n0p + 2 * k] = h->h_tb[k];
+    h->stage_x[n0p + 2 * k + 1] = 0.0 * h->h_tb[k] + h->ub[0]; h->stage_t[n0p + 2 * k + 1] = h->h_tb[k];
   }
   if (n_aux) {
     CUDA_TRY(cudaMemcpyAsync(h->d_x + h->dcap - n_aux, h->stage_x.data(), n_aux * 8, cudaMemcpyHostToDevice, h->stream));

@@ -80,7 +80,9 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 #define PINN_TANH_NEWTON1 1               // one Newton step on the reciprocal seed instead of two: the residual correction of the
 #endif                                    // quotient squares the remaining error once more (measured: <= 4 ulp kept, -1 % kernel time)
 __device__ __forceinline__ double tanh_fast(double x) {
-  const double ax = fmin(fabs(x), 20.0);        // tanh(20) rounds to 1.0
+  // tanh(20) rounds to 1.0.  A NaN fails the test and flows through to copysign (NaN in, NaN out, as libm); fmin would return
+  // 20 and make it +-1.  The compiler folds the select after -2|x|, so the FP64-pipe instruction counts are fmin's.
+  const double ax = fabs(x) > 20.0 ? 20.0 : fabs(x);
   const double y = -2.0 * ax;
   const double SHIFT = 6755399441055744.0;      // 1.5 * 2^52: round-to-nearest-integer trick
   const double t = fma(y, 1.4426950408889634, SHIFT);

@@ -3,7 +3,8 @@
 import collections, os, re, subprocess, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "pinns-tf2.0_b200", "lib", "libpinn_b200.so")
-WANT = ["burgers215fused_loss_grad", "3nls15fused_loss_grad", "7generic15fused_loss_grad", "reduce_tail", "adam_update", "lbfgs_iterateILi12ELi256", "lbfgs_dots", "lbfgs_solve", "lbfgs_apply"]
+WANT = ["burgers215fused_loss_grad", "7burgers15fused_loss_grad", "3nls15fused_loss_grad", "7generic15fused_loss_grad",
+        "4nsid15fused_loss_grad", "reduce_tail", "adam_update", "lbfgs_iterateILi12ELi256", "lbfgs_dots", "lbfgs_solve", "lbfgs_apply"]
 sass = subprocess.run(["cuobjdump", "-sass", LIB], capture_output=True, text=True).stdout
 res = subprocess.run(["cuobjdump", "-res-usage", LIB], capture_output=True, text=True).stdout
 usage = {m.group(1): m.group(2) for m in re.finditer(r"Function (\S+?):\s*\n\s*(REG:\d+ STACK:\d+ SHARED:\d+)", res)}

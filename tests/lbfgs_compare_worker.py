@@ -97,4 +97,27 @@ try:
     raise SystemExit("the reference was expected to fail with UnboundLocalError")
 except UnboundLocalError:
     print("%-34s reference raises UnboundLocalError (t unassigned); port reports 'no progress'" % "no progress at iteration 1")
+
+# Objectives whose f, g or both turn NaN or +-Inf at evaluation 0, 1 or 4 (tests/test_gpu_nonfinite.py holds the device L-BFGS
+# to the port on the same set): stop reason, counts, logged iterations and every point asked for, NaN-aware.
+sys.path.insert(0, ROOT + "/tests")
+from test_gpu_nonfinite import LBFGS_KW, LBFGS_OBJECTIVES, LBFGS_X0, nonfinite_objective  # noqa: E402
+for name, k, at, wh in LBFGS_OBJECTIVES:
+    kw = dict(maxIter=LBFGS_KW["max_iter"], learningRate=LBFGS_KW["lr"], nCorrection=LBFGS_KW["n_corr"], tolFun=LBFGS_KW["tol_fun"])
+    with np.errstate(all="ignore"):
+        port = rp.lbfgs_fixed_step(nonfinite_objective(k, at, wh), LBFGS_X0, max_iter=kw["maxIter"], learning_rate=kw["learningRate"],
+                                   n_correction=kw["nCorrection"], tol_fun=kw["tolFun"])
+        ret, xs, logged, said, state = run_reference(nonfinite_objective(k, at, wh), LBFGS_X0, verbose=True, **kw)
+    assert REASON_TEXT[port.stop_reason] in said, (name, port.stop_reason, said)
+    assert len(xs) == len(port.x_eval) == port.n_eval, (name, len(xs), port.n_eval)
+    for a, b in zip(xs, port.x_eval):
+        assert np.allclose(a, b, rtol=1e-8, atol=1e-13, equal_nan=True), name
+    if port.stop_reason == "initial optimality":
+        continue
+    x, f_hist, n_eval = ret
+    assert n_eval == port.n_eval and np.allclose(np.asarray(x), port.x_final, rtol=1e-8, atol=1e-13, equal_nan=True), name
+    assert np.allclose([float(v) for v in f_hist], port.f_hist, rtol=1e-8, atol=1e-300, equal_nan=True), name
+    assert [it for it, _ in logged] == [it for it, _ in port.logged], (name, logged, port.logged)
+    assert state.nIter == port.n_iter, (name, state.nIter, port.n_iter)
+print("%-34s %d objectives, reason, counts and points equal (NaN-aware)" % ("non-finite f / g", len(LBFGS_OBJECTIVES)))
 print("lbfgs control flow identical")

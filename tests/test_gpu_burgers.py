@@ -186,6 +186,17 @@ def test_device_tanh_accuracy(cabi):
     assert ulp.max() <= 4.0
     assert got[-3] == 1.0 and got[-2] == -1.0 and got[-4] == 0.0
     assert np.array_equal(cabi.device_tanh(-xs), -got)
+    # non-finite and edge inputs: quiet NaNs of both signs with payloads give NaN (libm's tanh), +-Inf and +-(20 +- ulp) give
+    # exactly +-1, +-0 keeps its sign, the smallest denormal stays within 4 ulp
+    nans = np.array([0x7FF8000000000000, 0xFFF8000000000000, 0x7FF800000000BEEF, 0xFFFC0000DEAD0001], dtype=np.uint64).view(np.float64)
+    assert np.all(np.isnan(cabi.device_tanh(nans)))
+    sat = np.array([np.inf, -np.inf, 20.0, -20.0, np.nextafter(20.0, 0), -np.nextafter(20.0, 0), np.nextafter(20.0, 30),
+                    -np.nextafter(20.0, 30)])
+    assert np.array_equal(cabi.device_tanh(sat), np.sign(sat))
+    z = cabi.device_tanh(np.array([0.0, -0.0]))
+    assert np.array_equal(z, [0.0, 0.0]) and not np.signbit(z[0]) and np.signbit(z[1])
+    tiny = np.array([5e-324, -5e-324])
+    assert np.all(np.abs(cabi.device_tanh(tiny) - np.tanh(tiny)) <= 4 * 5e-324)
 
 
 def test_zero_copy_collocation_matches_copied_and_sees_host_updates(cabi):
