@@ -55,6 +55,14 @@
 // profiles/experiments/burgers_chain_slotwise.patch).  Bit-identical, 51 instead of 13 DMMA.16x8x4 next to FP64 arithmetic in
 // the SASS, and 0.5 % slower: DMMA.16x8 interleaved with DFMA in one warp costs more than the latency it hides.  Fully
 // unrolled layer loops (no spills; 9-11 k instead of 7 k SASS instructions): forward +5 %, backward +1 %, both +18 %.
+// Backward ring wait, Z-bar staging and arrive moved after the input-adjoint DMMA issue (the counterpart of the forward
+// staging under the GEMM, which is kept): +5 %, the weight-gradient warps get Z-bar later.
+// Every chain GEMM moved to warps 4-7, each running a quarter of it (profiles/experiments/burgers_dmma_warps.patch): the chain
+// warps keep only the elementwise work and hand the staged operands over by mbarrier; the DMMA warps poll every chain's requests
+// and the weight-gradient tasks in their fixed order.  Bit-identical, no hang, 186 registers, no stack -- and 2.4 times slower
+// (0.747 against 0.305 ms; the input-adjoint GEMMs alone moved: 0.470 ms).  One DMMA warp per sub-partition now serves 56
+// requests per round one after another, ~500 cycles each (operand LDS, 5 dependent DMMAs, stores, hand-off), so its busy time
+// alone exceeds the whole kernel's; the chain warps spend most of their time waiting for GEMM results (DESIGN §6).
 #pragma once
 #include "burgers_fused.cuh"
 
@@ -458,12 +466,6 @@ __global__ void __maxnreg__(252) fused_loss_grad(const Args p) {
       }
       act_forward5(V);
       pc.mark(PH_FWD_ACT);
-      // the stash is still the A operand of the previous tile's weight-gradient tasks: wait until its last one, the layer-1
-      // task (J = 6), has been consumed; consumers retire tasks in order
-      if (it > 0) wait_consumed(bars, c, 7 * (it - 1) + 6);
-      pc.mark(PH_WAIT);
-      stage5(stash, V, lane);
-      pc.mark(PH_FWD_ACT);
       // ---------------- hidden layers 1..7: DMMA chain
 #pragma unroll 1
       for (int l = 1; l < NHID; l++) {
@@ -478,10 +480,18 @@ __global__ void __maxnreg__(252) fused_loss_grad(const Args p) {
             Z[1][nt][e] = Z[2][nt][e] = Z[3][nt][e] = 0.0;
           }
         if (!PINN_ABL_NODMMA) mma_layer5(Z, V, Wl, W, 1, lane);
+        // The outputs of layer l-1 (V, the GEMM's A operand in registers) go to the stash while the DMMAs run: the stores, and for
+        // l = 1 the wait below, sit under the GEMM instead of in series before it.  The stash is still the A operand of the
+        // previous tile's weight-gradient tasks; slot 0 is read by the last of them, the layer-1 task (J = 6), and consumers
+        // retire tasks in order, so once it is consumed every slot is free.
+        pc.mark(PH_FWD_GEMM);
+        if (l == 1 && it > 0) wait_consumed(bars, c, 7 * (it - 1) + 6);
+        pc.mark(PH_WAIT);
+        stage5(stash + (l - 1) * STASHL, V, lane);                  // STASH0 == STASHL
+        pc.mark(PH_FWD_ACT);
         c_to_v5(V, Z, lane);
         pc.mark(PH_FWD_GEMM);
         act_forward5(V);
-        if (l < NHID - 1) stage5(stash + STASH0 + (l - 1) * STASHL, V, lane);
         pc.mark(PH_FWD_ACT);
       }
       // ---------------- output layer (20 -> 1), residual, seeds
