@@ -14,7 +14,11 @@
  *     C-contiguous;
  *   - the handle owns all device memory, one CUDA stream and (world > 1) one NCCL communicator; it is not
  *     thread-safe; one process per GPU;
- *   - functions that return a host scalar/array synchronise the handle's stream; the others only enqueue.
+ *   - functions that return a host scalar/array synchronise the handle's stream; the others only enqueue;
+ *   - what a handle returns depends only on its CURRENT inputs (points, targets, constants, stage matrices, residual spec,
+ *     source, weights, optimiser state), never on the calls that brought it there: after any order of setter, evaluation and
+ *     optimiser calls it equals, bit for bit, a fresh handle fed the same inputs, and a refused call changes nothing
+ *     (tests/test_gpu_handle_state.py).
  *
  * Flat parameter layout (utils/neuralnetwork.py:68-89 get_weights/set_weights, :97-100 flat gradient):
  *   for each Dense layer in order: W.flatten() (row-major [in,out]) then b;  identification appends
@@ -192,7 +196,8 @@ int pinn_lbfgs(pinn_t* h, int max_iter, double learning_rate, int n_correction, 
 
 /* f_hist of the last pinn_lbfgs run (custom_lbfgs.py:66-67,186-187: the initial f and the f of every evaluation, including
  * the ones that hit a stop test and were therefore not logged).  *n_out = number of evaluations; f_hist_out may be NULL to
- * query the count. */
+ * query the count.  pinn_lbfgs(max_iter = 0) is a run too (lbfgs() returns before it evaluates anything): the history is
+ * empty after it, not that of the run before. */
 int pinn_lbfgs_history(pinn_t* h, double* f_hist_out, int capacity, int* n_out);
 
 /* lbfgs() for an ARBITRARY opfunc (utils/custom_lbfgs.py:39-236 takes any closure x -> (f, g)): a stand-alone device-resident

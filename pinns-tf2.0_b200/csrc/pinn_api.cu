@@ -1278,7 +1278,7 @@ int pinn_lbfgs(pinn_t* h, int max_iter, double learning_rate, int n_correction, 
   if (n_iter_out) *n_iter_out = 0;
   if (n_eval_out) *n_eval_out = 0;
   if (reason_out) *reason_out = PINN_LBFGS_RUNNING;
-  if (max_iter == 0) return 0;                                      // custom_lbfgs.py:43-44
+  if (max_iter == 0) { h->lb_fhist.clear(); return 0; }             // custom_lbfgs.py:43-44: a run with no evaluation
   if (max_iter < 0) return fail("pinn_lbfgs: max_iter < 0");
   if (n_correction <= 0) n_correction = 100;                        // :52 (`or 100`)
   if (n_correction > 128) return fail("pinn_lbfgs: n_correction > 128 not supported");

@@ -232,7 +232,8 @@ def test_zero_copy_collocation_matches_copied_and_sees_host_updates(cabi):
 
 def test_mapped_collocation_first_then_growing_data_block(cabi):
     """Regression (ADVICE r1): a fresh handle whose ONLY collocation set is a zero-copy mapping has no device collocation
-    region (capacity 0); growing the data block afterwards must not copy n_c doubles out of it."""
+    region (capacity 0); growing the data block afterwards must not copy n_c doubles out of it.  (Now one case of the seeded
+    histories of tests/test_gpu_handle_state.py: "data region regrown under a mapped batch".)"""
     import ctypes as C
     rng = np.random.default_rng(21)
     lb, ub = np.array([-1.0, 0.0]), np.array([1.0, 0.99])
@@ -261,7 +262,7 @@ def test_mapped_collocation_first_then_growing_data_block(cabi):
 
 def test_residual_buffer_is_sized_by_the_library(cabi):
     """pinn_residual takes the row count of the caller's buffer and refuses a mismatch (ADVICE r1: it used to write n_c rows
-    into whatever it was given)."""
+    into whatever it was given).  (That a refused call leaves the handle as it was is tests/test_gpu_handle_state.py's.)"""
     import ctypes as C
     g = load_golden("burgers_inf")
     p = make_inf(cabi, g)
