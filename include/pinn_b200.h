@@ -80,7 +80,8 @@ const char* pinn_version(void);
 
 /* NeuralNetwork.__init__ (utils/neuralnetwork.py:8-47): layers = hp["layers"]; lb/ub feed the normalising
  * Lambda (:29-30).  rank/world/nccl_uid: data-parallel sharding of the collocation set (new capability,
- * SURVEY 8(e)); nccl_uid = 128-byte ncclUniqueId from pinn_nccl_unique_id on rank 0, NULL when world==1.
+ * SURVEY 8(e)); nccl_uid = 128-byte ncclUniqueId from pinn_nccl_unique_id on rank 0, NULL when world==1.  world > 1 is
+ * accepted for BURGERS_INF and NLS_INF only (DESIGN.md section 5).
  * lb and ub hold max(2, layers[0]) entries: (x, t), or (x, y, t) for NS_IDE. */
 int pinn_create(pinn_t** out, int pde_id, int n_layers, const int* layers, const double* lb, const double* ub,
                 int device, int rank, int world, const void* nccl_uid);

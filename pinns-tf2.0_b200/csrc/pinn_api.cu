@@ -758,6 +758,15 @@ int pinn_create(pinn_t** out, int pde_id, int n_layers, const int* layers, const
   if (pde_id < 0 || pde_id > 9) return fail("pinn_create: unknown pde_id");
   const bool ns = pde_id == PINN_NS_IDE;
   if (ns && world > 1) return fail("pinn_create: the Navier-Stokes identification model runs on one GPU (world must be 1)");
+  // Sharding (utils/sharding.py) splits the collocation rows with the global 1/N_f and weights the replicated terms by the data
+  // weight.  The discrete-time heads have no collocation set and sum every term without a data weight, and Burgers
+  // identification puts its residual on the data points with the local 1/n_d: sharded, each of them counts the wrong loss.
+  if (world > 1 && (pde_id == PINN_BURGERS_IDE || is_disc(pde_id)))
+    return fail(pde_id == PINN_BURGERS_IDE
+                    ? "pinn_create: the Burgers identification model runs on one GPU (world must be 1): its residual sits on the data "
+                      "points, which carry no data weight"
+                    : "pinn_create: the discrete-time models run on one GPU (world must be 1): they have no collocation set to shard "
+                      "and their heads read no data weight");
   if (is_poly(pde_id)) {
     if (world > 1) return fail("pinn_create: the polynomial residual models run on one GPU (world must be 1)");
     if (layers[0] != 2 || layers[n_layers - 1] != 1)
