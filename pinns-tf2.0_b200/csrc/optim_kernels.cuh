@@ -26,9 +26,60 @@ struct LbfgsState {
   int free_slot;    // physical slot that receives the candidate pair of the next iteration
   int apply;        // what lbfgs_apply has to do: 0 nothing, 1 move the model weights, 2 write x_final (last iteration)
   int slot[129];    // physical slot of the pair of age i (0 = oldest), i < k
-  double c_g, step; // direction d = c_g g + sum_m ca[m] s_m + cb[m] y_m  (m = age), step length t
+  double c_g;       // direction d = c_g g + sum_m ca[m] s_m + cb[m] y_m  (m = age)
   double ca[128], cb[128];
 };
+
+// ------------------------------------------------------------------------------------------------
+// The rules of the reference routine (utils/custom_lbfgs.py:39-236) that both L-BFGS formulations below share.
+// ------------------------------------------------------------------------------------------------
+// Stop tests of the evaluation that has just completed, in the reference's order: initial optimality after the first
+// evaluation (:65-76), then max_eval (:195), optimality (:200-204), step below tolX (:206-210) and f change below tolX
+// (:212-215).  g1 = |g|_1, s1 = |d t|_1 (not read for the initial evaluation).  Returns the status, 0 = keep going.
+__device__ __forceinline__ int lbfgs_eval_status(const LbfgsState* st, int n_iter, int n_eval, double g1, double s1, double f_new) {
+  if (n_iter == 0) return g1 <= st->tol_fun ? 7 : 0;
+  if ((double)n_eval >= st->max_eval) return 2;
+  if (g1 <= st->tol_fun) return 3;
+  if (s1 <= st->tol_x) return 4;
+  if (fabs(f_new - st->f_old) < st->tol_x) return 5;
+  return 0;
+}
+
+// Thread 0's record of that evaluation: f_hist, and the log flag of its iteration (:217-218: an iteration is logged after its
+// stop tests, and only if none of them fired).
+__device__ __forceinline__ void lbfgs_record_eval(LbfgsState* st, int n_iter, int n_eval, double f_new, int status,
+                                                  double* f_hist, int* logged) {
+  st->n_eval = n_eval;
+  st->f = f_new;
+  st->pending = 0;
+  f_hist[n_eval - 1] = f_new;
+  if (n_iter > 0 && status == 0) logged[n_iter] = 1;
+  st->status = status;
+}
+
+// The step of iteration n_iter from g.d and |g|_1: no progress along d stops the run (:154-156, status 6); the step length
+// is min(1, 1/|g|_1) on the first iteration and the fixed learning rate after (:159-163); the last iteration's update goes
+// to x_final instead of the model and is never evaluated (:176-182, status 1 at :192).
+struct LbfgsStep {
+  bool stop, last;
+  double t;
+};
+__device__ __forceinline__ LbfgsStep lbfgs_step(const LbfgsState* st, int n_iter, double gtd, double g1) {
+  LbfgsStep s;
+  s.stop = gtd > -st->tol_x;
+  s.t = (n_iter == 1) ? fmin(1.0, 1.0 / g1) : st->lr;
+  s.last = n_iter == st->max_iter;
+  return s;
+}
+// Thread 0's record of the step (f_old = f precedes the progress test, :144-145).
+__device__ __forceinline__ void lbfgs_record_step(LbfgsState* st, int n_iter, const LbfgsStep& s) {
+  st->n_iter = n_iter;
+  st->f_old = st->f;
+  if (s.stop) { st->status = 6; return; }
+  st->t = s.t;
+  if (s.last) st->status = 1;
+  else st->pending = 1;
+}
 
 // ------------------------------------------------------------------------------------------------
 // reduce the per-CTA partial vectors (fixed order -> deterministic).  src index map: gradient entries
@@ -350,11 +401,9 @@ lbfgs_iterate(LbfgsState* __restrict__ st, double* __restrict__ w, const double*
 #pragma unroll
     for (int e = 0; e < EPT; e++) a1 += fabs(gv[e]);
     a1 = block_sum(a1, red);
-    int status = 0;
-    if (n_iter == 0) {
-      // initial evaluation (custom_lbfgs.py:65-76)
-      if (a1 <= st->tol_fun) status = 7;
-    } else {
+    int status;
+    if (n_iter == 0) status = lbfgs_eval_status(st, n_iter, n_eval, a1, 0.0, f_new);   // no step yet, so no |d t|_1
+    else {
       double a2 = 0.0;
       const double t = st->t;
 #pragma unroll
@@ -363,20 +412,10 @@ lbfgs_iterate(LbfgsState* __restrict__ st, double* __restrict__ w, const double*
         a2 += i < P ? fabs(d[i] * t) : 0.0;
       }
       a2 = block_sum(a2, red);
-      if ((double)n_eval >= st->max_eval) status = 2;                    // :195
-      else if (a1 <= st->tol_fun) status = 3;                            // :200-204
-      else if (a2 <= st->tol_x) status = 4;                              // :206-210
-      else if (fabs(f_new - st->f_old) < st->tol_x) status = 5;          // :212-215
+      status = lbfgs_eval_status(st, n_iter, n_eval, a1, a2, f_new);
     }
     __syncthreads();
-    if (tid == 0) {
-      st->n_eval = n_eval;
-      st->f = f_new;
-      st->pending = 0;
-      f_hist[n_eval - 1] = f_new;
-      if (n_iter > 0 && status == 0) logged[n_iter] = 1;                 // :217-218 (log after the stop tests)
-      st->status = status;
-    }
+    if (tid == 0) lbfgs_record_eval(st, n_iter, n_eval, f_new, status, f_hist, logged);
     __syncthreads();
     if (status != 0) return;
   }
@@ -506,31 +545,20 @@ lbfgs_iterate(LbfgsState* __restrict__ st, double* __restrict__ w, const double*
     const int i = tid + e * LB_THREADS;
     if (i < P) { g_old[i] = gv[e]; d[i] = dv[e]; }
   }
-  const double f_cur = st->f;
-  if (gtd > -st->tol_x) {                                                // :154-156
-    __syncthreads();
-    if (tid == 0) { st->n_iter = n_iter; st->f_old = f_cur; st->status = 6; }
-    return;
-  }
-  const double t = (n_iter == 1) ? fmin(1.0, 1.0 / a1) : st->lr;         // :159-163
-  const bool last = (n_iter == st->max_iter);
+  const LbfgsStep step = lbfgs_step(st, n_iter, gtd, a1);
+  if (!step.stop) {
 #pragma unroll
-  for (int e = 0; e < EPT; e++) {
-    const int i = tid + e * LB_THREADS;
-    if (i < P) {
-      const double xn = w[i] + t * dv[e];                                // :174
-      if (last) x_final[i] = xn;       // no evaluation follows (:176-182): the model keeps the previous weights
-      else w[i] = xn;
+    for (int e = 0; e < EPT; e++) {
+      const int i = tid + e * LB_THREADS;
+      if (i < P) {
+        const double xn = w[i] + step.t * dv[e];                         // :174
+        if (step.last) x_final[i] = xn;
+        else w[i] = xn;
+      }
     }
   }
   __syncthreads();
-  if (tid == 0) {
-    st->n_iter = n_iter;
-    st->f_old = f_cur;
-    st->t = t;
-    if (last) st->status = 1;                                            // :192
-    else st->pending = 1;
-  }
+  if (tid == 0) lbfgs_record_step(st, n_iter, step);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -641,24 +669,13 @@ lbfgs_solve(LbfgsState* __restrict__ st, const double* __restrict__ R, int P, co
   const double f_new = R[P] + R[P + 1] + R[P + 2];
   const double a1 = dots[0];
   const int NS = st->n_corr + 1;
-  // ---- (a) bookkeeping + stop tests of the evaluation that has just completed (custom_lbfgs.py:65-76, 186-218)
+  // ---- (a) bookkeeping + stop tests of the evaluation that has just completed
   if (st->pending) {
     const int n_iter = st->n_iter, n_eval = st->n_eval + 1;
-    int status = 0;
-    if (n_iter == 0) {
-      if (a1 <= st->tol_fun) status = 7;
-    } else {
-      if ((double)n_eval >= st->max_eval) status = 2;                    // :195
-      else if (a1 <= st->tol_fun) status = 3;                            // :200-204
-      else if (dots[2] <= st->tol_x) status = 4;                         // :206-210
-      else if (fabs(f_new - st->f_old) < st->tol_x) status = 5;          // :212-215
-    }
+    const int status = lbfgs_eval_status(st, n_iter, n_eval, a1, dots[2], f_new);
     __syncthreads();
     if (tid == 0) {
-      st->n_eval = n_eval; st->f = f_new; st->pending = 0;
-      f_hist[n_eval - 1] = f_new;
-      if (n_iter > 0 && status == 0) logged[n_iter] = 1;                 // :217-218 (log after the stop tests)
-      st->status = status;
+      lbfgs_record_eval(st, n_iter, n_eval, f_new, status, f_hist, logged);
       if (status != 0) st->apply = 0;
     }
     if (status != 0) return;
@@ -753,20 +770,12 @@ lbfgs_solve(LbfgsState* __restrict__ st, const double* __restrict__ R, int P, co
     if (tid == 0) { st->c_g = -h_diag; st->k = k; st->h_diag = h_diag; st->free_slot = free_next; }
   }
   if (n_iter == 1 && tid == 0) { st->k = 0; st->free_slot = 0; }
-  // ---- (c) step (:144-182)
+  // ---- (c) step
   __syncthreads();
   if (tid == 0) {
-    const double f_cur = st->f;
-    if (gtd > -st->tol_x) {                                              // :154-156
-      st->n_iter = n_iter; st->f_old = f_cur; st->status = 6; st->apply = 0;
-    } else {
-      const double t = (n_iter == 1) ? fmin(1.0, 1.0 / a1) : st->lr;     // :159-163
-      const bool last = (n_iter == st->max_iter);
-      st->step = t; st->t = t; st->n_iter = n_iter; st->f_old = f_cur;
-      st->apply = last ? 2 : 1;
-      if (last) st->status = 1;                                          // :192
-      else st->pending = 1;
-    }
+    const LbfgsStep step = lbfgs_step(st, n_iter, gtd, a1);
+    lbfgs_record_step(st, n_iter, step);
+    st->apply = step.stop ? 0 : step.last ? 2 : 1;
   }
 }
 
@@ -791,7 +800,7 @@ lbfgs_apply(LbfgsState* __restrict__ st, double* __restrict__ w, const double* _
     dv = fma(cb[m], Y[o], dv);
   }
   g_old[i] = gi; d[i] = dv;                // :144, the direction of this step (s of the next iteration = d t)
-  const double xn = fma(st->step, dv, w[i]);                             // :174
+  const double xn = fma(st->t, dv, w[i]);                                // :174
   if (apply == 2) x_final[i] = xn;         // no evaluation follows (:176-182): the model keeps the previous weights
   else w[i] = xn;
 }

@@ -72,8 +72,128 @@ constexpr int NCCL_SUM = 0;       // ncclSum
 
 constexpr int LOSS_RING = 4096;
 
-// buffers of the Gram-matrix L-BFGS formulation (optim_kernels.cuh: lbfgs_dots / lbfgs_solve / lbfgs_apply)
-struct LbfgsGram { double *SY = nullptr, *YY = nullptr, *part = nullptr; int n_corr_cap = 0, n_blocks = 0, stride = 0; };
+// One L-BFGS iteration on the device (stop tests of the pending evaluation, history update, direction, step).
+// Default: the single-CTA kernel that follows the reference's loop literally (lbfgs_iterate).
+// PINN_LBFGS=gram selects the Gram-matrix formulation (lbfgs_dots -> lbfgs_solve -> lbfgs_apply: every SM reads its slice of
+// the history, so it takes less time per iteration, and it has no 32768-entry limit).  It is not the default: the literal
+// kernel is the reference's loop term by term.  Long fixed-step runs diverge from some starting points in BOTH modes
+// (profiles/lbfgs_stability_h100.jsonl); the step-by-step replay in tests/test_gpu_optimizer_replay.py keeps both kernels
+// within their fp64 error bound up to the divergence (DESIGN.md section 4.3).
+bool lbfgs_serial() {
+  static int v = -1;
+  if (v < 0) { const char* e = getenv("PINN_LBFGS"); v = (e && !strcmp(e, "gram")) ? 0 : 1; }
+  return v == 1;
+}
+
+// The arguments of one L-BFGS run after the reference's defaults (utils/custom_lbfgs.py:49-55).
+struct LbfgsConfig {
+  int max_iter, n_corr;
+  double lr, tol_fun, tol_x, max_eval;
+};
+
+// Applies those defaults to the caller's arguments (0 = default) and refuses what the device kernels cannot run: more than
+// 128 history pairs, more than 32768 entries in the single-CTA kernel.  `who` names the entry point in the messages.
+int lbfgs_config(const char* who, int64_t n, int max_iter, double lr, int n_corr, double tol_fun, double tol_x, double max_eval,
+                 LbfgsConfig* c) {
+  const std::string w(who);
+  if (lbfgs_serial() && n > 32 * 1024) return fail(w + ": vector too large for the single-CTA L-BFGS kernel (32768 entries)");
+  if (n > (1 << 30)) return fail(w + ": vector too large");
+  if (n_corr <= 0) n_corr = 100;                                             // :52 (`or 100`)
+  if (n_corr > 128) return fail(w + ": n_correction > 128 not supported");
+  *c = LbfgsConfig{max_iter, n_corr, lr == 0.0 ? 1.0 : lr,                   // :55
+                   tol_fun == 0.0 ? 1e-5 : tol_fun,                          // :50
+                   tol_x == 0.0 ? 1e-19 : tol_x,                             // :51
+                   max_eval == 0.0 ? max_iter * 1.25 : max_eval};            // :49
+  return 0;
+}
+
+// Iterations whose stop tests have run: all < n_iter, plus n_iter itself unless its evaluation is pending.
+int lbfgs_tested(const pinn::LbfgsState& s) { return s.pending ? s.n_iter - 1 : s.n_iter; }
+
+// The device state of L-BFGS runs (optim_kernels.cuh): the LbfgsState, the vectors of an iteration, the (s, y) history ring,
+// f_hist, the per-iteration log flags and the Gram formulation's buffers.  The buffers only grow, so an owner that runs
+// L-BFGS again reuses them.
+struct DeviceLbfgs {
+  pinn::LbfgsState* st = nullptr;
+  double *g_old = nullptr, *d = nullptr, *x_final = nullptr, *S = nullptr, *Y = nullptr, *f_hist = nullptr;
+  int* logged = nullptr;
+  double *SY = nullptr, *YY = nullptr, *part = nullptr;   // Gram formulation (lbfgs_dots / lbfgs_solve / lbfgs_apply)
+  int n_cap = 0, corr_cap = 0, iter_cap = 0, part_stride = 0;
+
+  int reserve(int n, int n_corr, int max_iter) {
+    if (!st) CUDA_TRY(cudaMalloc((void**)&st, sizeof(pinn::LbfgsState)));
+    if (n > n_cap || n_corr > corr_cap) {
+      if (n < n_cap) n = n_cap;
+      if (n_corr < corr_cap) n_corr = corr_cap;
+      for (double* b : {g_old, d, x_final, S, Y, SY, YY, part}) if (b) cudaFree(b);
+      g_old = d = x_final = S = Y = SY = YY = part = nullptr;
+      const size_t NS = (size_t)n_corr + 1;                 // + the spare history slot of the Gram formulation
+      const size_t nb = (n + pinn::LB_CHUNK - 1) / pinn::LB_CHUNK;
+      part_stride = pinn::LB_NSCAL + 4 * n_corr + 1;
+      CUDA_TRY(cudaMalloc((void**)&g_old, (size_t)n * 8));
+      CUDA_TRY(cudaMalloc((void**)&d, (size_t)n * 8));
+      CUDA_TRY(cudaMalloc((void**)&x_final, (size_t)n * 8));
+      CUDA_TRY(cudaMalloc((void**)&S, NS * n * 8));
+      CUDA_TRY(cudaMalloc((void**)&Y, NS * n * 8));
+      CUDA_TRY(cudaMalloc((void**)&SY, NS * NS * 8));
+      CUDA_TRY(cudaMalloc((void**)&YY, NS * NS * 8));
+      CUDA_TRY(cudaMalloc((void**)&part, nb * part_stride * 8));
+      if ((size_t)n_corr * n_corr * 8 > 48 * 1024)
+        CUDA_TRY(cudaFuncSetAttribute(pinn::lbfgs_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, n_corr * n_corr * 8));
+      n_cap = n; corr_cap = n_corr;
+    }
+    if (max_iter + 2 > iter_cap) {
+      if (f_hist) cudaFree(f_hist);
+      if (logged) cudaFree(logged);
+      f_hist = nullptr; logged = nullptr;
+      CUDA_TRY(cudaMalloc((void**)&f_hist, (size_t)(max_iter + 2) * 8));
+      CUDA_TRY(cudaMalloc((void**)&logged, (size_t)(max_iter + 2) * 4));
+      iter_cap = max_iter + 2;
+    }
+    return 0;
+  }
+
+  // Clears f_hist and the log flags and writes the initial state of a run (after reserve).
+  int start(cudaStream_t stream, const LbfgsConfig& c) {
+    CUDA_TRY(cudaMemsetAsync(logged, 0, (size_t)(c.max_iter + 2) * 4, stream));
+    CUDA_TRY(cudaMemsetAsync(f_hist, 0, (size_t)(c.max_iter + 2) * 8, stream));
+    pinn::LbfgsState s{};
+    s.pending = 1;                               // the initial evaluation comes first
+    s.max_iter = c.max_iter; s.n_corr = c.n_corr; s.max_eval = c.max_eval;
+    s.lr = c.lr; s.tol_fun = c.tol_fun; s.tol_x = c.tol_x; s.h_diag = 1.0;
+    CUDA_TRY(cudaMemcpyAsync(st, &s, sizeof(s), cudaMemcpyHostToDevice, stream));
+    CUDA_TRY(cudaStreamSynchronize(stream));     // s is a stack object
+    return 0;
+  }
+
+  // One iteration on the P-vector w, whose gradient and loss parts are R = [g | 3 loss parts].
+  int iterate(cudaStream_t stream, double* w, const double* R, int P, long long* launches) const {
+    if (lbfgs_serial()) {
+#define LB_LAUNCH(E, NT) pinn::lbfgs_iterate<E, NT><<<1, NT, 0, stream>>>(st, w, R, P, g_old, d, S, Y, x_final, f_hist, logged)
+      if (P <= 12 * 256) LB_LAUNCH(12, 256);        // Burgers-size vectors: 8 warps, 12 entries per thread
+      else if (P <= 8 * 1024) LB_LAUNCH(8, 1024);
+      else LB_LAUNCH(32, 1024);
+#undef LB_LAUNCH
+      if (cudaGetLastError() != cudaSuccess) return fail("lbfgs_iterate launch failed");
+      if (launches) *launches += 1;
+      return 0;
+    }
+    const int nb = (P + pinn::LB_CHUNK - 1) / pinn::LB_CHUNK;
+    pinn::lbfgs_dots<<<nb, pinn::LB_DOT_THREADS, 0, stream>>>(st, R, P, g_old, d, S, Y, part, part_stride);
+    pinn::lbfgs_solve<<<1, 128, (size_t)corr_cap * corr_cap * 8, stream>>>(st, R, P, part, nb, part_stride, SY, YY, f_hist, logged);
+    pinn::lbfgs_apply<<<nb, pinn::LB_CHUNK, 0, stream>>>(st, w, R, P, g_old, d, S, Y, x_final);
+    if (cudaGetLastError() != cudaSuccess) return fail("L-BFGS iteration launch failed");
+    if (launches) *launches += 3;
+    return 0;
+  }
+
+  void release() {
+    for (double* b : {g_old, d, x_final, S, Y, f_hist, SY, YY, part}) if (b) cudaFree(b);
+    if (logged) cudaFree(logged);
+    if (st) cudaFree(st);
+    *this = DeviceLbfgs{};
+  }
+};
 
 }  // namespace
 
@@ -133,11 +253,7 @@ struct pinn_handle {
   size_t flush_bytes = 0;
 
   // L-BFGS
-  pinn::LbfgsState* d_lb = nullptr;
-  double *d_gold = nullptr, *d_d = nullptr, *d_S = nullptr, *d_Y = nullptr, *d_xfinal = nullptr, *d_fhist = nullptr;
-  int* d_logged = nullptr;
-  int lb_corr_cap = 0, lb_iter_cap = 0;
-  LbfgsGram lb_gram;
+  DeviceLbfgs lbfgs;
   std::vector<double> lb_fhist;             // f of every evaluation of the last pinn_lbfgs run (custom_lbfgs.py f_hist)
 
   // scratch for predict / derivatives
@@ -190,64 +306,6 @@ int nls_launch_eval(pinn_t* h, const int* run_flag);
 int generic_launch_eval(pinn_t* h, const int* run_flag);
 int ns_launch_eval(pinn_t* h, const int* run_flag);
 int disc_upload_points(pinn_t* h);
-
-// One L-BFGS iteration on the device (stop tests of the pending evaluation, history update, direction, step).
-// Default: the single-CTA kernel that follows the reference's loop literally (lbfgs_iterate).
-// PINN_LBFGS=gram selects the Gram-matrix formulation (lbfgs_dots -> lbfgs_solve -> lbfgs_apply: every SM reads its slice of
-// the history, so it takes less time per iteration, and it has no 32768-entry limit).  It is not the default: the literal
-// kernel is the reference's loop term by term.  Long fixed-step runs diverge from some starting points in BOTH modes
-// (profiles/lbfgs_stability_h100.jsonl); the step-by-step replay in tests/test_gpu_optimizer_replay.py keeps both kernels
-// within their fp64 error bound up to the divergence (DESIGN.md section 4.3).
-bool lbfgs_serial() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("PINN_LBFGS"); v = (e && !strcmp(e, "gram")) ? 0 : 1; }
-  return v == 1;
-}
-int lbfgs_gram_ensure(LbfgsGram* gm, int n_corr, int P) {
-  const int nb = (P + pinn::LB_CHUNK - 1) / pinn::LB_CHUNK;
-  if (n_corr <= gm->n_corr_cap && nb <= gm->n_blocks) return 0;
-  if (gm->SY) cudaFree(gm->SY);
-  if (gm->YY) cudaFree(gm->YY);
-  if (gm->part) cudaFree(gm->part);
-  gm->SY = gm->YY = gm->part = nullptr;
-  const size_t NS = (size_t)n_corr + 1;
-  gm->stride = pinn::LB_NSCAL + 4 * n_corr + 1;
-  if (cudaMalloc((void**)&gm->SY, NS * NS * 8) != cudaSuccess || cudaMalloc((void**)&gm->YY, NS * NS * 8) != cudaSuccess ||
-      cudaMalloc((void**)&gm->part, (size_t)nb * gm->stride * 8) != cudaSuccess)
-    return fail("cudaMalloc failed (L-BFGS Gram buffers)");
-  gm->n_corr_cap = n_corr; gm->n_blocks = nb;
-  if ((size_t)n_corr * n_corr * 8 > 48 * 1024 &&
-      cudaFuncSetAttribute(pinn::lbfgs_solve, cudaFuncAttributeMaxDynamicSharedMemorySize, n_corr * n_corr * 8) != cudaSuccess)
-    return fail("cudaFuncSetAttribute(lbfgs_solve) failed");
-  return 0;
-}
-void lbfgs_gram_free(LbfgsGram* gm) {
-  if (gm->SY) cudaFree(gm->SY);
-  if (gm->YY) cudaFree(gm->YY);
-  if (gm->part) cudaFree(gm->part);
-  *gm = LbfgsGram{};
-}
-int lbfgs_launch_iteration(cudaStream_t stream, pinn::LbfgsState* st, double* w, const double* R, int P, double* gold, double* d,
-                           double* S, double* Y, double* xfinal, double* fhist, int* logged, const LbfgsGram& gm, long long* launches) {
-  if (lbfgs_serial()) {
-#define LB_LAUNCH(E, NT) pinn::lbfgs_iterate<E, NT><<<1, NT, 0, stream>>>(st, w, R, P, gold, d, S, Y, xfinal, fhist, logged)
-    if (P <= 12 * 256) LB_LAUNCH(12, 256);        // Burgers-size vectors: 8 warps, 12 entries per thread
-    else if (P <= 8 * 1024) LB_LAUNCH(8, 1024);
-    else LB_LAUNCH(32, 1024);
-#undef LB_LAUNCH
-    if (cudaGetLastError() != cudaSuccess) return fail("lbfgs_iterate launch failed");
-    if (launches) *launches += 1;
-    return 0;
-  }
-  const int nb = (P + pinn::LB_CHUNK - 1) / pinn::LB_CHUNK;
-  pinn::lbfgs_dots<<<nb, pinn::LB_DOT_THREADS, 0, stream>>>(st, R, P, gold, d, S, Y, gm.part, gm.stride);
-  pinn::lbfgs_solve<<<1, 128, (size_t)gm.n_corr_cap * gm.n_corr_cap * 8, stream>>>(st, R, P, gm.part, nb, gm.stride, gm.SY, gm.YY, fhist,
-                                                                                   logged);
-  pinn::lbfgs_apply<<<nb, pinn::LB_CHUNK, 0, stream>>>(st, w, R, P, gold, d, S, Y, xfinal);
-  if (cudaGetLastError() != cudaSuccess) return fail("L-BFGS iteration launch failed");
-  if (launches) *launches += 3;
-  return 0;
-}
 
 // after a stream synchronisation: has the fused P2P exchange reported a peer that never published?
 int check_p2p(pinn_t* h) {
@@ -857,8 +915,6 @@ int pinn_create(pinn_t** out, int pde_id, int n_layers, const int* layers, const
   CREATE_TRY(cudaMemset(h->d_step, 0, 16));
   CREATE_TRY(cudaMalloc((void**)&h->d_loss_ring, LOSS_RING * 8));
   CREATE_TRY(cudaMemset(h->d_loss_ring, 0, LOSS_RING * 8));
-  CREATE_TRY(cudaMalloc((void**)&h->d_lb, sizeof(pinn::LbfgsState)));
-  CREATE_TRY(cudaMemset(h->d_lb, 0, sizeof(pinn::LbfgsState)));
   if (h->kernel_kind == 3) {
     h->n_cta = h->n_sm;
     h->pstride = ((h->P_net + 8 + 15) / 16) * 16;
@@ -907,13 +963,11 @@ int pinn_destroy(pinn_t* h) {
   if (h->d_p2p_err) cudaFree(h->d_p2p_err);
   if (h->d_xseq) cudaFree(h->d_xseq);
   if (h->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(h->comm);
-  double* bufs[] = {h->d_w, h->d_R, h->d_partials, h->d_m, h->d_v, h->d_loss_ring, h->d_x, h->d_t, h->d_u, h->d_scrH, h->d_scrA, h->d_scrS, h->d_gH, h->d_gA, h->d_gS, h->d_irk, h->d_gold,
-                    h->d_d, h->d_S, h->d_Y, h->d_xfinal, h->d_fhist, h->d_px, h->d_pout, h->d_pscr, h->d_nsX, h->d_src};
+  double* bufs[] = {h->d_w, h->d_R, h->d_partials, h->d_m, h->d_v, h->d_loss_ring, h->d_x, h->d_t, h->d_u, h->d_scrH, h->d_scrA, h->d_scrS, h->d_gH, h->d_gA, h->d_gS, h->d_irk,
+                    h->d_px, h->d_pout, h->d_pscr, h->d_nsX, h->d_src};
   for (double* b : bufs) if (b) cudaFree(b);
   if (h->d_step) cudaFree(h->d_step);
-  if (h->d_lb) cudaFree(h->d_lb);
-  if (h->d_logged) cudaFree(h->d_logged);
-  lbfgs_gram_free(&h->lb_gram);
+  h->lbfgs.release();
   for (cudaEvent_t e : h->events) cudaEventDestroy(e);
   if (h->d_flush) cudaFree(h->d_flush);
   if (h->ev0) cudaEventDestroy(h->ev0);
@@ -1289,69 +1343,31 @@ int pinn_lbfgs(pinn_t* h, int max_iter, double learning_rate, int n_correction, 
   if (reason_out) *reason_out = PINN_LBFGS_RUNNING;
   if (max_iter == 0) { h->lb_fhist.clear(); return 0; }             // custom_lbfgs.py:43-44: a run with no evaluation
   if (max_iter < 0) return fail("pinn_lbfgs: max_iter < 0");
-  if (n_correction <= 0) n_correction = 100;                        // :52 (`or 100`)
-  if (n_correction > 128) return fail("pinn_lbfgs: n_correction > 128 not supported");
-  if (learning_rate == 0.0) learning_rate = 1.0;                    // :55
-  if (tol_fun == 0.0) tol_fun = 1e-5;                               // :50
-  if (tol_x == 0.0) tol_x = 1e-19;                                  // :51
-  if (sync_every < 1) sync_every = 1;
   const int P = h->P;
-  if (lbfgs_serial() && P > 32 * 1024) return fail("pinn_lbfgs: parameter vector too large for the single-CTA L-BFGS kernel");
+  LbfgsConfig cfg;
+  if (lbfgs_config("pinn_lbfgs", P, max_iter, learning_rate, n_correction, tol_fun, tol_x, 0.0, &cfg)) return -1;
+  if (sync_every < 1) sync_every = 1;
   CUDA_TRY(cudaSetDevice(h->device));
-  if (!h->d_gold) {
-    CUDA_TRY(cudaMalloc((void**)&h->d_gold, h->w_cap * 8));
-    CUDA_TRY(cudaMalloc((void**)&h->d_d, h->w_cap * 8));
-    CUDA_TRY(cudaMalloc((void**)&h->d_xfinal, h->w_cap * 8));
-  }
-  if (n_correction > h->lb_corr_cap) {
-    if (h->d_S) cudaFree(h->d_S);
-    if (h->d_Y) cudaFree(h->d_Y);
-    h->d_S = h->d_Y = nullptr;
-    CUDA_TRY(cudaMalloc((void**)&h->d_S, (size_t)(n_correction + 1) * P * 8));     // + the spare slot of the Gram formulation
-    CUDA_TRY(cudaMalloc((void**)&h->d_Y, (size_t)(n_correction + 1) * P * 8));
-    h->lb_corr_cap = n_correction;
-  }
-  if (lbfgs_gram_ensure(&h->lb_gram, n_correction, P)) return -1;
-  if (max_iter + 2 > h->lb_iter_cap) {
-    if (h->d_fhist) cudaFree(h->d_fhist);
-    if (h->d_logged) cudaFree(h->d_logged);
-    h->d_fhist = nullptr; h->d_logged = nullptr;
-    CUDA_TRY(cudaMalloc((void**)&h->d_fhist, (size_t)(max_iter + 2) * 8));
-    CUDA_TRY(cudaMalloc((void**)&h->d_logged, (size_t)(max_iter + 2) * 4));
-    h->lb_iter_cap = max_iter + 2;
-  }
-  CUDA_TRY(cudaMemsetAsync(h->d_logged, 0, (size_t)(max_iter + 2) * 4, h->stream));
-  CUDA_TRY(cudaMemsetAsync(h->d_fhist, 0, (size_t)(max_iter + 2) * 8, h->stream));
-  pinn::LbfgsState st{};
-  st.status = 0; st.n_iter = 0; st.n_eval = 0; st.k = 0; st.head = 0; st.pending = 1;
-  st.max_iter = max_iter; st.n_corr = n_correction;
-  st.max_eval = max_iter * 1.25;                                    // :49
-  st.lr = learning_rate; st.tol_fun = tol_fun; st.tol_x = tol_x;
-  st.h_diag = 1.0; st.t = 0.0; st.f = 0.0; st.f_old = 0.0;
-  CUDA_TRY(cudaMemcpyAsync(h->d_lb, &st, sizeof(st), cudaMemcpyHostToDevice, h->stream));
-  CUDA_TRY(cudaStreamSynchronize(h->stream));   // st is a stack object
-  const int* run_flag = &h->d_lb->status;
+  DeviceLbfgs& lb = h->lbfgs;
+  if (lb.reserve(P, cfg.n_corr, max_iter) || lb.start(h->stream, cfg)) return -1;
+  const int* run_flag = &lb.st->status;
   if (launch_eval(h, run_flag)) return -1;      // initial f, g (:65)
 
   std::vector<double> fh(max_iter + 2);
   std::vector<int> lg(max_iter + 2);
+  pinn::LbfgsState st{};
   int reported = 0;
-  auto iterate = [&]() -> int {
-    return lbfgs_launch_iteration(h->stream, h->d_lb, h->d_w, h->d_R, P, h->d_gold, h->d_d, h->d_S, h->d_Y, h->d_xfinal, h->d_fhist,
-                                  h->d_logged, h->lb_gram, &h->launches);
-  };
   while (true) {
     for (int b = 0; b < sync_every; b++) {
-      if (iterate()) return -1;
+      if (lb.iterate(h->stream, h->d_w, h->d_R, P, &h->launches)) return -1;
       if (launch_eval(h, run_flag)) return -1;
     }
-    CUDA_TRY(cudaMemcpyAsync(&st, h->d_lb, sizeof(st), cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(cudaMemcpyAsync(fh.data(), h->d_fhist, (size_t)(max_iter + 2) * 8, cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(cudaMemcpyAsync(lg.data(), h->d_logged, (size_t)(max_iter + 2) * 4, cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(cudaMemcpyAsync(&st, lb.st, sizeof(st), cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(cudaMemcpyAsync(fh.data(), lb.f_hist, (size_t)(max_iter + 2) * 8, cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(cudaMemcpyAsync(lg.data(), lb.logged, (size_t)(max_iter + 2) * 4, cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(cudaStreamSynchronize(h->stream));
     if (check_p2p(h)) return -1;
-    // iterations whose stop tests have run: all < n_iter, plus n_iter itself unless its evaluation is pending
-    const int upto = st.pending ? st.n_iter - 1 : st.n_iter;
+    const int upto = lbfgs_tested(st);
     for (int it = reported + 1; it <= upto; it++)
       if (lg[it] && log_cb) log_cb(it, fh[it], user);
     if (upto > reported) reported = upto;
@@ -1364,7 +1380,7 @@ int pinn_lbfgs(pinn_t* h, int max_iter, double learning_rate, int n_correction, 
   if (x_final_or_null) {
     // x after the loop: differs from the model weights only when the loop ended on max_iter (the last update
     // is not evaluated, utils/custom_lbfgs.py:176-182; utils/neuralnetwork.py:131-136 ignores the return).
-    const double* src = (st.status == PINN_LBFGS_MAX_ITER) ? h->d_xfinal : h->d_w;
+    const double* src = (st.status == PINN_LBFGS_MAX_ITER) ? lb.x_final : h->d_w;
     CUDA_TRY(cudaMemcpyAsync(x_final_or_null, src, (size_t)P * 8, cudaMemcpyDeviceToHost, h->stream));
     CUDA_TRY(cudaStreamSynchronize(h->stream));
   }
@@ -1619,16 +1635,13 @@ int pinn_kernel_info(pinn_t* h, char* buf, int buflen) {
 // -----------------------------------------------------------------------------------------------------------------
 // Stand-alone device-resident L-BFGS for ANY objective (utils/custom_lbfgs.py:39 takes an arbitrary `opfunc`): the caller
 // evaluates f and g wherever it likes and feeds them in; the vectors, the (s, y) history ring and the two-loop recursion
-// stay on the device and run through the SAME kernel (lbfgs_iterate) the PINN handles use.
+// stay on the device and run through the SAME kernels (DeviceLbfgs) the PINN handles use.
 // -----------------------------------------------------------------------------------------------------------------
 struct pinn_lbfgs_handle {
-  int device = 0, n = 0, max_iter = 0, n_corr = 0;
+  int device = 0, n = 0;
   cudaStream_t stream = nullptr;
-  pinn::LbfgsState* d_st = nullptr;
-  double *d_x = nullptr, *d_R = nullptr, *d_gold = nullptr, *d_d = nullptr, *d_S = nullptr, *d_Y = nullptr, *d_xfinal = nullptr,
-         *d_fhist = nullptr;
-  int* d_logged = nullptr;
-  LbfgsGram gram;
+  double *d_x = nullptr, *d_R = nullptr;   // the iterate; [g | f 0 0], laid out as a model's reduced vector
+  DeviceLbfgs lb;
   int reported = 0;
 };
 
@@ -1636,11 +1649,9 @@ int pinn_lbfgs_destroy(pinn_lbfgs_t* s) {
   if (!s) return 0;
   cudaSetDevice(s->device);
   if (s->stream) cudaStreamSynchronize(s->stream);
-  double* bufs[] = {s->d_x, s->d_R, s->d_gold, s->d_d, s->d_S, s->d_Y, s->d_xfinal, s->d_fhist};
-  for (double* b : bufs) if (b) cudaFree(b);
-  if (s->d_logged) cudaFree(s->d_logged);
-  lbfgs_gram_free(&s->gram);
-  if (s->d_st) cudaFree(s->d_st);
+  if (s->d_x) cudaFree(s->d_x);
+  if (s->d_R) cudaFree(s->d_R);
+  s->lb.release();
   if (s->stream) cudaStreamDestroy(s->stream);
   delete s;
   return 0;
@@ -1650,48 +1661,25 @@ int pinn_lbfgs_create(pinn_lbfgs_t** out, int device, int64_t n, const double* x
                       int n_correction, double tol_fun, double tol_x, double max_eval) {
   if (!out || !x0 || n < 1) return fail("pinn_lbfgs_create: bad arguments");
   if (max_iter < 1) return fail("pinn_lbfgs_create: max_iter must be >= 1 (lbfgs() returns before anything for maxIter == 0)");
-  if (lbfgs_serial() && n > 32 * 1024) return fail("pinn_lbfgs_create: vector too large for the single-CTA L-BFGS kernel (32768 entries)");
-  if (n > (1 << 30)) return fail("pinn_lbfgs_create: vector too large");
-  if (n_correction <= 0) n_correction = 100;                        // custom_lbfgs.py:52
-  if (n_correction > 128) return fail("pinn_lbfgs_create: n_correction > 128 not supported");
-  if (learning_rate == 0.0) learning_rate = 1.0;                    // :55
-  if (tol_fun == 0.0) tol_fun = 1e-5;                               // :50
-  if (tol_x == 0.0) tol_x = 1e-19;                                  // :51
-  if (max_eval == 0.0) max_eval = max_iter * 1.25;                  // :49
+  LbfgsConfig cfg;
+  if (lbfgs_config("pinn_lbfgs_create", n, max_iter, learning_rate, n_correction, tol_fun, tol_x, max_eval, &cfg)) return -1;
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail("pinn_lbfgs_create: no CUDA device -- this library has no CPU fallback");
   if (device < 0 || device >= ndev) return fail("pinn_lbfgs_create: bad device index");
   pinn_lbfgs_t* s = new pinn_lbfgs_t();
-  s->device = device; s->n = (int)n; s->max_iter = max_iter; s->n_corr = n_correction;
-#define LB_TRY(expr)                                                                                     \
-  do {                                                                                                   \
-    cudaError_t _e = (expr);                                                                             \
-    if (_e != cudaSuccess) { fail(std::string(#expr) + ": " + cudaGetErrorString(_e)); pinn_lbfgs_destroy(s); return -1; } \
-  } while (0)
-  LB_TRY(cudaSetDevice(device));
-  LB_TRY(cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking));
-  const size_t nb = ((size_t)n + 8) * 8;
-  LB_TRY(cudaMalloc((void**)&s->d_x, nb));
-  LB_TRY(cudaMalloc((void**)&s->d_R, nb));
-  LB_TRY(cudaMalloc((void**)&s->d_gold, nb));
-  LB_TRY(cudaMalloc((void**)&s->d_d, nb));
-  LB_TRY(cudaMalloc((void**)&s->d_xfinal, nb));
-  LB_TRY(cudaMalloc((void**)&s->d_S, (size_t)(n_correction + 1) * n * 8));
-  LB_TRY(cudaMalloc((void**)&s->d_Y, (size_t)(n_correction + 1) * n * 8));
-  if (lbfgs_gram_ensure(&s->gram, n_correction, (int)n)) { pinn_lbfgs_destroy(s); return -1; }
-  LB_TRY(cudaMalloc((void**)&s->d_fhist, (size_t)(max_iter + 2) * 8));
-  LB_TRY(cudaMalloc((void**)&s->d_logged, (size_t)(max_iter + 2) * 4));
-  LB_TRY(cudaMalloc((void**)&s->d_st, sizeof(pinn::LbfgsState)));
-  LB_TRY(cudaMemsetAsync(s->d_fhist, 0, (size_t)(max_iter + 2) * 8, s->stream));
-  LB_TRY(cudaMemsetAsync(s->d_logged, 0, (size_t)(max_iter + 2) * 4, s->stream));
-  LB_TRY(cudaMemsetAsync(s->d_R, 0, nb, s->stream));
-  LB_TRY(cudaMemcpyAsync(s->d_x, x0, (size_t)n * 8, cudaMemcpyHostToDevice, s->stream));
-  pinn::LbfgsState st{};
-  st.pending = 1; st.max_iter = max_iter; st.n_corr = n_correction; st.max_eval = max_eval;
-  st.lr = learning_rate; st.tol_fun = tol_fun; st.tol_x = tol_x; st.h_diag = 1.0;
-  LB_TRY(cudaMemcpyAsync(s->d_st, &st, sizeof(st), cudaMemcpyHostToDevice, s->stream));
-  LB_TRY(cudaStreamSynchronize(s->stream));
-#undef LB_TRY
+  s->device = device; s->n = (int)n;
+  auto setup = [&]() -> int {
+    CUDA_TRY(cudaSetDevice(device));
+    CUDA_TRY(cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking));
+    const size_t nb = ((size_t)n + 8) * 8;
+    CUDA_TRY(cudaMalloc((void**)&s->d_x, nb));
+    CUDA_TRY(cudaMalloc((void**)&s->d_R, nb));
+    CUDA_TRY(cudaMemsetAsync(s->d_R, 0, nb, s->stream));
+    CUDA_TRY(cudaMemcpyAsync(s->d_x, x0, (size_t)n * 8, cudaMemcpyHostToDevice, s->stream));
+    if (s->lb.reserve((int)n, cfg.n_corr, max_iter)) return -1;
+    return s->lb.start(s->stream, cfg);
+  };
+  if (setup()) { pinn_lbfgs_destroy(s); return -1; }
   *out = s;
   return 0;
 }
@@ -1704,30 +1692,29 @@ int pinn_lbfgs_feed(pinn_lbfgs_t* s, double f, const double* g, double* x_next, 
   const double tail[3] = {f, 0.0, 0.0};          // the kernel reads f as the sum of three loss parts behind the gradient
   CUDA_TRY(cudaMemcpyAsync(s->d_R, g, (size_t)n * 8, cudaMemcpyHostToDevice, s->stream));
   CUDA_TRY(cudaMemcpyAsync(s->d_R + n, tail, 24, cudaMemcpyHostToDevice, s->stream));
-  if (lbfgs_launch_iteration(s->stream, s->d_st, s->d_x, s->d_R, n, s->d_gold, s->d_d, s->d_S, s->d_Y, s->d_xfinal, s->d_fhist,
-                             s->d_logged, s->gram, nullptr)) return -1;
+  if (s->lb.iterate(s->stream, s->d_x, s->d_R, n, nullptr)) return -1;
   pinn::LbfgsState st{};
-  CUDA_TRY(cudaMemcpyAsync(&st, s->d_st, sizeof(st), cudaMemcpyDeviceToHost, s->stream));
+  CUDA_TRY(cudaMemcpyAsync(&st, s->lb.st, sizeof(st), cudaMemcpyDeviceToHost, s->stream));
   CUDA_TRY(cudaStreamSynchronize(s->stream));
   *status_out = st.status;
   if (n_iter_out) *n_iter_out = st.n_iter;
   if (n_eval_out) *n_eval_out = st.n_eval;
   // the iteration whose stop tests have just run (custom_lbfgs.py:217-218 logs it only if none of them fired)
-  const int tested = st.pending ? st.n_iter - 1 : st.n_iter;
+  const int tested = lbfgs_tested(st);
   int logged_it = -1;
   double logged_f = 0.0;
   // (at most one iteration is newly logged per evaluation; when the loop ends on max_iter, `tested` also covers the final,
   // never-evaluated and never-logged iteration)
   for (int it = s->reported + 1; it <= tested && it >= 1; it++) {
     int flag = 0;
-    CUDA_TRY(cudaMemcpy(&flag, s->d_logged + it, 4, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(&flag, s->lb.logged + it, 4, cudaMemcpyDeviceToHost));
     if (flag) { logged_it = it; logged_f = f; }
   }
   if (tested > s->reported) s->reported = tested;
   if (logged_iter_out) *logged_iter_out = logged_it;
   if (logged_f_out) *logged_f_out = logged_f;
   // where to evaluate next (status 0), or the vector lbfgs() returns: the last update when the loop ended on max_iter
-  const double* src = (st.status == PINN_LBFGS_MAX_ITER) ? s->d_xfinal : s->d_x;
+  const double* src = (st.status == PINN_LBFGS_MAX_ITER) ? s->lb.x_final : s->d_x;
   CUDA_TRY(cudaMemcpy(x_next, src, (size_t)n * 8, cudaMemcpyDeviceToHost));
   return 0;
 }
@@ -1736,11 +1723,11 @@ int pinn_lbfgs_f_hist(pinn_lbfgs_t* s, double* f_hist_out, int capacity, int* n_
   if (!s || !n_out) return fail("pinn_lbfgs_f_hist: null argument");
   CUDA_TRY(cudaSetDevice(s->device));
   pinn::LbfgsState st{};
-  CUDA_TRY(cudaMemcpy(&st, s->d_st, sizeof(st), cudaMemcpyDeviceToHost));
+  CUDA_TRY(cudaMemcpy(&st, s->lb.st, sizeof(st), cudaMemcpyDeviceToHost));
   *n_out = st.n_eval;
   if (f_hist_out) {
     if (capacity < st.n_eval) return fail("pinn_lbfgs_f_hist: buffer too small");
-    if (st.n_eval) CUDA_TRY(cudaMemcpy(f_hist_out, s->d_fhist, (size_t)st.n_eval * 8, cudaMemcpyDeviceToHost));
+    if (st.n_eval) CUDA_TRY(cudaMemcpy(f_hist_out, s->lb.f_hist, (size_t)st.n_eval * 8, cudaMemcpyDeviceToHost));
   }
   return 0;
 }

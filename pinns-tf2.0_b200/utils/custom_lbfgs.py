@@ -5,12 +5,14 @@ two-loop kernel (pinn_lbfgs in include/pinn_b200.h).
 (custom_lbfgs.py:39-44,76,236).  When ``opfunc`` is the closure returned by ``NeuralNetwork.get_loss_and_flat_grad`` the
 whole iteration (evaluation, history update, two-loop recursion, fixed step, stop tests) runs on the GPU with one status
 read-back per ``sync_every`` iterations instead of the reference's >= 6 host syncs per iteration.  Any OTHER closure is
-called once per iteration, as in the reference, while the optimiser state stays on the device (``_lbfgs_foreign``).
+called once per iteration, as in the reference, while the optimiser state stays on the device (``_run_foreign``).
 There is deliberately no host (CPU) implementation of the optimiser arithmetic.
 """
 import time
 
 import numpy as np
+
+import pinn_cabi
 
 # ---- wall-time bookkeeping (custom_lbfgs.py:8-28)
 global_time_list = []
@@ -57,21 +59,30 @@ class Struct(dummy):
         return self.__dict__.get(key, 0)
 
 
-def _lbfgs_foreign(opfunc, x, config, state, do_verbose, log_fn):
+def _run_coupled(net, x, config, max_iter, opts, on_logged):
+    """The closure of NeuralNetwork.get_loss_and_flat_grad: evaluations and iterations both run on the device, with one
+    status read-back per ``sync_every`` iterations."""
+    sync_every = int(config.syncEvery or getattr(getattr(net, "logger", None), "frequency", 1) or 1)
+    net.set_weights(x)
+    logged = []
+
+    def _cb(it, f):
+        logged.append((it, f))
+        on_logged(it, f)
+
+    res = net._native().lbfgs(max_iter, sync_every=max(1, sync_every), log_fn=_cb, want_x_final=True, **opts)
+    f_hist = res.get("f_hist", [f for _, f in logged])
+    return net._as_tensor(res["x_final"]), f_hist, res["n_iter"], res["n_eval"], res["reason"]
+
+
+def _run_foreign(opfunc, x, config, max_iter, opts, on_logged):
     """Any closure x -> (f, g) (custom_lbfgs.py:39): the objective is evaluated by the caller's code, one call per iteration
     exactly where the reference calls it (:65, :178), while the iterate, the (s, y) history and the two-loop recursion stay
-    on the device (pinn_lbfgs_create / pinn_lbfgs_feed -- the same kernel as the fused training path).  x is handed to opfunc
+    on the device (pinn_lbfgs_create / pinn_lbfgs_feed -- the same kernels as the coupled path).  x is handed to opfunc
     as a float64 array with .numpy(); f and g may be anything np.asarray() understands."""
-    global final_loss, times
-    import pinn_cabi
     from neuralnetwork import _t
-    max_iter = int(config.maxIter)
-    if config.lineSearch:
-        raise NotImplementedError("lineSearch is dead code in the reference (custom_lbfgs.py:168-171) and is not provided")
     x0 = np.asarray(x.numpy() if hasattr(x, "numpy") else x, dtype=np.float64).reshape(-1)
-    opt = pinn_cabi.Lbfgs(x0, max_iter, learning_rate=float(config.learningRate or 1), n_correction=int(config.nCorrection or 100),
-                          tol_fun=float(config.tolFun or 1e-5), tol_x=float(config.tolX or 1e-19), max_eval=float(config.maxEval or 0.0))
-    times = []
+    opt = pinn_cabi.Lbfgs(x0, max_iter, max_eval=float(config.maxEval or 0.0), **opts)
     try:
         xk = x0
         while True:
@@ -80,63 +91,45 @@ def _lbfgs_foreign(opfunc, x, config, state, do_verbose, log_fn):
             g = np.asarray(g.numpy() if hasattr(g, "numpy") else g, dtype=np.float64).reshape(-1)
             xk, status, n_iter, n_eval, logged_it, logged_f = opt.feed(f, g)
             if logged_it is not None:
-                if do_verbose:
-                    log_fn(logged_it, np.float64(logged_f), True)
-                    record_time()
-                    times.append(last_time())
-                if logged_it == max_iter - 1:
-                    final_loss = np.float64(logged_f)
+                on_logged(logged_it, logged_f)
             if status != 0:
                 break
         f_hist = opt.f_hist()
     finally:
         opt.close()
-    state.funcEval = state.funcEval + n_eval
-    state.nIter = state.nIter + n_iter
-    state.stop_reason = pinn_cabi.LBFGS_REASONS.get(status, "?")
-    if status == 7:             # initial optimality (custom_lbfgs.py:73-76)
-        return _t(xk), f_hist
-    return _t(xk), f_hist, n_eval
+    return _t(xk), f_hist, n_iter, n_eval, status
 
 
 def lbfgs(opfunc, x, config, state, do_verbose, log_fn):
     """Device-resident port of the reference control flow.  Returns None when maxIter == 0, ``(x, f_hist)`` when
     the initial point is already optimal, else ``(x, f_hist, currentFuncEval)``."""
-    global final_loss, times
+    global times
     if config.maxIter == 0:
         return
-    net = getattr(opfunc, "_pinn_net", None)
-    if net is None:
-        return _lbfgs_foreign(opfunc, x, config, state, do_verbose, log_fn)
-    max_iter = int(config.maxIter)
-    tol_fun = config.tolFun or 1e-5
-    tol_x = config.tolX or 1e-19
-    n_corr = int(config.nCorrection or 100)
-    lr = config.learningRate or 1
     if config.lineSearch:
         raise NotImplementedError("lineSearch is dead code in the reference (custom_lbfgs.py:168-171) and is not provided")
-    sync_every = int(config.syncEvery or getattr(getattr(net, "logger", None), "frequency", 1) or 1)
-
-    net.set_weights(x)
+    max_iter = int(config.maxIter)
+    opts = dict(learning_rate=float(config.learningRate or 1), n_correction=int(config.nCorrection or 100),
+                tol_fun=float(config.tolFun or 1e-5), tol_x=float(config.tolX or 1e-19))
     times = []
-    logged = []
 
-    def _cb(it, f):
-        logged.append((it, f))
+    def on_logged(it, f):
+        global final_loss
         if do_verbose:
             log_fn(it, np.float64(f), True)
             record_time()
             times.append(last_time())
         if it == max_iter - 1:
-            globals()["final_loss"] = np.float64(f)
+            final_loss = np.float64(f)
 
-    res = net._native().lbfgs(max_iter, learning_rate=float(lr), n_correction=n_corr, tol_fun=float(tol_fun),
-                              tol_x=float(tol_x), sync_every=max(1, sync_every), log_fn=_cb, want_x_final=True)
-    state.funcEval = state.funcEval + res["n_eval"]
-    state.nIter = state.nIter + res["n_iter"]
-    state.stop_reason = res["reason_str"]
-    f_hist = res.get("f_hist", [f for _, f in logged])
-    x_out = net._as_tensor(res["x_final"])
-    if res["reason"] == 7:      # initial optimality (custom_lbfgs.py:73-76)
+    net = getattr(opfunc, "_pinn_net", None)
+    if net is not None:
+        x_out, f_hist, n_iter, n_eval, reason = _run_coupled(net, x, config, max_iter, opts, on_logged)
+    else:
+        x_out, f_hist, n_iter, n_eval, reason = _run_foreign(opfunc, x, config, max_iter, opts, on_logged)
+    state.funcEval = state.funcEval + n_eval
+    state.nIter = state.nIter + n_iter
+    state.stop_reason = pinn_cabi.LBFGS_REASONS.get(reason, "?")
+    if reason == 7:             # initial optimality (custom_lbfgs.py:73-76)
         return x_out, f_hist
-    return x_out, f_hist, res["n_eval"]
+    return x_out, f_hist, n_eval
