@@ -195,6 +195,37 @@ struct DeviceLbfgs {
   }
 };
 
+// The fused loss/gradient kernel a handle runs, chosen once in pinn_create.
+enum class Kernel {
+  BurgersV2,      // specialised Burgers DMMA kernel, warp-specialised (default for the Burgers net)
+  BurgersV1,      // specialised Burgers DMMA kernel, single-role (PINN_BURGERS_KERNEL=v1)
+  Schrodinger,    // specialised NLS DMMA kernel
+  Generic,        // any other layer list, and the discrete-time and polynomial residual heads
+  NavierStokes,
+};
+
+// Grow-only per-CTA scratch of the generic, Schrodinger and Navier-Stokes kernels (activations, adjoints, seeds).  A handle
+// runs one kernel, so one set serves it; it is regrown only when the points per CTA exceed those it was sized for.
+struct Scratch {
+  double *H = nullptr, *A = nullptr, *S = nullptr;
+  long long pts = 0;
+
+  int reserve(long long pts_per_cta, size_t h_bytes, size_t a_bytes, size_t s_bytes) {
+    if (pts_per_cta <= pts) return 0;
+    release();
+    CUDA_TRY(cudaMalloc((void**)&H, h_bytes));
+    CUDA_TRY(cudaMalloc((void**)&A, a_bytes));
+    CUDA_TRY(cudaMalloc((void**)&S, s_bytes));
+    pts = pts_per_cta;
+    return 0;
+  }
+
+  void release() {
+    for (double* b : {H, A, S}) if (b) cudaFree(b);
+    *this = Scratch{};
+  }
+};
+
 }  // namespace
 
 struct pinn_handle {
@@ -213,12 +244,10 @@ struct pinn_handle {
   int n_sm = 0;
   long long launches = 0;
   bool tail_inflight = false;   // a launch with the in-kernel tail may still be running on this handle's stream
-  pinn::ReduceMap last_map{};       // reduction map / grid / stride of the most recent fused launch
+  pinn::ReduceMap last_map{};       // reduction map / grid / stride of the most recent fused launch (record_launch)
   int last_grid = 0, last_stride = 0;
-  int kernel_kind = 0;              // 0: specialised Burgers DMMA kernel, 1: specialised NLS DMMA kernel, 2: generic, 3: Navier-Stokes
-  double *d_gH = nullptr, *d_gA = nullptr, *d_gS = nullptr;   // generic kernel scratch
-  long long g_pts = 0;
-  int burgers_kernel = 2;           // 2: warp-specialised (default); 1: single-role v1 (PINN_BURGERS_KERNEL=v1)
+  Kernel kernel = Kernel::Generic;
+  Scratch scratch;
 
   // parameters and optimiser state
   double* d_w = nullptr;            // WPAD-padded flat weights
@@ -243,9 +272,7 @@ struct pinn_handle {
   std::vector<double> h_icx, h_ict;         // NLS initial-condition points (host copy for re-assembly)
   const double *map_x = nullptr, *map_t = nullptr;   // zero-copy collocation block (device aliases of pinned host memory)
   long long n_aux = 0;                      // points stored in the data region (Burgers: n_d; NLS: n0p + 2 n_b)
-  double *d_scrH = nullptr, *d_scrA = nullptr, *d_scrS = nullptr;   // NLS activation / adjoint / seed scratch
-  int scr_pts = 0;
-  std::vector<double> stage_x, stage_t;     // host staging for set_data (de-interleave)
+  std::vector<double> stage_x, stage_t;     // host staging of the data-region block (upload_points)
 
   // measurement
   std::vector<cudaEvent_t> events;
@@ -282,13 +309,50 @@ struct pinn_handle {
 
 namespace {
 
-// 1-D (x only) discrete-time models; identification: two snapshots, q outputs; inference: q+1 outputs
-bool is_disc(int pde) { return pde == PINN_BURGERS_DISC || pde == PINN_BURGERS_IDE_DISC || pde == PINN_KDV_IDE_DISC || pde == PINN_AC_DISC; }
-bool is_ide_disc(int pde) { return pde == PINN_BURGERS_IDE_DISC || pde == PINN_KDV_IDE_DISC; }
-// user-defined polynomial residual (pinn_set_residual) on the generic kernel's POLY instantiation
-bool is_poly(int pde) { return pde == PINN_POLY_INF || pde == PINN_POLY_IDE; }
-// continuous-time models whose data points are also the residual points
-bool residual_on_data(int pde) { return pde == PINN_BURGERS_IDE || pde == PINN_NS_IDE || pde == PINN_POLY_IDE; }
+// What each model is, indexed by pde id.  Host code branches on these fields; a switch on the pde is left only where the models
+// compute different things (the residual formulas, the constants, the layout of a re-assembled point block).
+enum class Out { One, Two, QPlus1, Q };   // network outputs: exactly 1, exactly 2, q+1 >= 2 (IRK inference), q >= 1 (IRK identification)
+enum class Res { None, Data, Colloc };    // residual points: none (discrete-time), the data points, the collocation set
+
+struct Model {
+  int in_dim;             // 1: x, 2: (x, t), 3: (x, y, t)
+  Out out;
+  int head_cap;           // widest output layer (the IRK head may be q+1 = 501 wide)
+  int n_lambda;           // trained lambdas behind the net parameters: P = P_net + n_lambda
+  Res residual;           // Res::Colloc: the model has a collocation set (pinn_set_collocation); no other model has one
+  bool boundary;          // pinn_set_boundary
+  bool snapshots;         // two snapshots (pinn_set_snapshot)
+  bool irk;               // a stage matrix (pinn_set_irk)
+  bool poly;              // a user-defined polynomial residual (pinn_set_residual, pinn_set_source) on generic::fused_loss_grad<true>
+  Kernel kernel;          // the specialised kernel that runs the model's BASELINE net (Generic: none)
+  const char* no_shard;   // why world must be 1 (nullptr: the model may be sharded)
+};
+
+// Sharding (utils/sharding.py) splits the collocation rows with the global 1/N_f and weights the replicated terms by the data
+// weight.  The discrete-time heads have no collocation set and sum every term without a data weight, and Burgers
+// identification puts its residual on the data points with the local 1/n_d: sharded, each of them counts the wrong loss.
+constexpr const char* NO_SHARD_DISC = "pinn_create: the discrete-time models run on one GPU (world must be 1): they have no "
+                                      "collocation set to shard and their heads read no data weight";
+constexpr Model MODELS[10] = {
+    /* BURGERS_INF      */ {2, Out::One, pinn::MAXW_WIDE, 0, Res::Colloc, false, false, false, false, Kernel::BurgersV2, nullptr},
+    /* BURGERS_IDE      */ {2, Out::One, pinn::MAXW_WIDE, 2, Res::Data, false, false, false, false, Kernel::BurgersV2,
+                            "pinn_create: the Burgers identification model runs on one GPU (world must be 1): its residual sits on "
+                            "the data points, which carry no data weight"},
+    /* NLS_INF          */ {2, Out::Two, pinn::MAXW_WIDE, 0, Res::Colloc, true, false, false, false, Kernel::Schrodinger, nullptr},
+    /* BURGERS_DISC     */ {1, Out::QPlus1, 512, 0, Res::None, true, false, true, false, Kernel::Generic, NO_SHARD_DISC},
+    /* BURGERS_IDE_DISC */ {1, Out::Q, 512, 2, Res::None, false, true, true, false, Kernel::Generic, NO_SHARD_DISC},
+    /* KDV_IDE_DISC     */ {1, Out::Q, 512, 2, Res::None, false, true, true, false, Kernel::Generic, NO_SHARD_DISC},
+    /* AC_DISC          */ {1, Out::QPlus1, 512, 0, Res::None, false, false, true, false, Kernel::Generic, NO_SHARD_DISC},
+    /* NS_IDE           */ {3, Out::Two, pinn::MAXW_WIDE, 2, Res::Data, false, false, false, false, Kernel::NavierStokes,
+                            "pinn_create: the Navier-Stokes identification model runs on one GPU (world must be 1)"},
+    /* POLY_INF         */ {2, Out::One, pinn::MAXW_WIDE, 0, Res::Colloc, false, false, false, true, Kernel::Generic,
+                            "pinn_create: the polynomial residual models run on one GPU (world must be 1)"},
+    /* POLY_IDE         */ {2, Out::One, pinn::MAXW_WIDE, 2, Res::Data, false, false, false, true, Kernel::Generic,
+                            "pinn_create: the polynomial residual models run on one GPU (world must be 1)"},
+};
+static_assert(sizeof(MODELS) / sizeof(MODELS[0]) == PINN_POLY_IDE + 1, "one MODELS row per pde id");
+
+const Model& model(const pinn_t* h) { return MODELS[h->pde]; }
 
 bool is_burgers_net(const std::vector<int>& L) {
   if (L.size() != 10 || L[0] != 2 || L[9] != 1) return false;
@@ -301,11 +365,9 @@ bool is_nls_net(const std::vector<int>& L) {
   return true;
 }
 
-int nls_upload_points(pinn_t* h);
 int nls_launch_eval(pinn_t* h, const int* run_flag);
 int generic_launch_eval(pinn_t* h, const int* run_flag);
 int ns_launch_eval(pinn_t* h, const int* run_flag);
-int disc_upload_points(pinn_t* h);
 
 // after a stream synchronisation: has the fused P2P exchange reported a peer that never published?
 int check_p2p(pinn_t* h) {
@@ -371,6 +433,77 @@ int ensure_points(pinn_t* h, long long need_d, long long need_c) {
   return 0;
 }
 
+// Writes the staged block (stage_x, stage_t) right-aligned into the data region, growing the point arrays for it and for the
+// current collocation set first; kernel point 0 then sits at dcap - n_aux.
+int upload_points(pinn_t* h) {
+  const long long n = (long long)h->stage_x.size();
+  if (ensure_points(h, n, h->n_c)) return -1;
+  if (n) {
+    CUDA_TRY(cudaMemcpyAsync(h->d_x + h->dcap - n, h->stage_x.data(), n * 8, cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(cudaMemcpyAsync(h->d_t + h->dcap - n, h->stage_t.data(), n * 8, cudaMemcpyHostToDevice, h->stream));
+    CUDA_TRY(cudaStreamSynchronize(h->stream));
+  }
+  h->n_aux = n;
+  return 0;
+}
+
+// The data-region blocks that are re-assembled from host copies whenever one of their parts changes.
+//   Schrodinger: [initial-condition points | pad to even | (lb_k, ub_k) pairs] (inf_cont_schrodinger.py:50-53 builds
+//                X_lb = (0*tb+lb0, tb), X_ub = (0*tb+ub0, tb)); the pairs are adjacent and must not straddle a CTA.
+//   Allen-Cahn: [x_0 | pad to even | lb, ub]: the periodic pair starts at an even index, so it never straddles a CTA.
+//   other discrete-time models: [x_0 data points | x_1 boundary points or snapshot].  t is unused in all three 1-D layouts.
+int assemble_points(pinn_t* h) {
+  const long long n0 = h->n_d, n0p = (n0 + 1) & ~1LL;
+  std::vector<double> &x = h->stage_x, &t = h->stage_t;
+  switch (h->pde) {
+    case PINN_NLS_INF:
+      x.assign(n0p + 2 * h->n_b, 0.0); t.assign(x.size(), 0.0);
+      for (long long i = 0; i < n0; i++) { x[i] = h->h_icx[i]; t[i] = h->h_ict[i]; }
+      if (n0p > n0) { x[n0] = h->lb[0]; t[n0] = h->lb[1]; }     // inert alignment point
+      for (long long k = 0; k < h->n_b; k++) {
+        // x as the reference forms it, 0 * tb + lb0: NaN for an infinite or NaN tb, lb0 (ub0) for every finite one
+        x[n0p + 2 * k] = 0.0 * h->h_tb[k] + h->lb[0];     t[n0p + 2 * k] = h->h_tb[k];
+        x[n0p + 2 * k + 1] = 0.0 * h->h_tb[k] + h->ub[0]; t[n0p + 2 * k + 1] = h->h_tb[k];
+      }
+      break;
+    case PINN_AC_DISC:
+      x.assign(n0 > 0 ? n0p + 2 : 0, 0.0); t.assign(x.size(), 0.0);
+      for (long long i = 0; i < n0; i++) x[i] = h->h_x0[i];
+      if (n0 > 0) {
+        for (long long i = n0; i < n0p; i++) x[i] = h->lb[0];    // inert alignment point
+        x[n0p] = h->lb[0]; x[n0p + 1] = h->ub[0];
+      }
+      break;
+    default:
+      x.assign(n0 + h->n_b, 0.0); t.assign(x.size(), 0.0);
+      for (long long i = 0; i < n0; i++) x[i] = h->h_x0[i];
+      for (long long i = 0; i < h->n_b; i++) x[n0 + i] = h->h_tb[i];
+      break;
+  }
+  return upload_points(h);
+}
+
+// Copies n doubles from the caller's buffer into the grow-only device buffer *p and waits: the buffer is only borrowed.
+int upload(pinn_t* h, double** p, long long* cap, const double* src, long long n) {
+  if (n <= 0) return 0;
+  if (ensure(p, cap, n)) return -1;
+  CUDA_TRY(cudaMemcpyAsync(*p, src, n * 8, cudaMemcpyHostToDevice, h->stream));
+  CUDA_TRY(cudaStreamSynchronize(h->stream));
+  return 0;
+}
+
+// Records h's most recent fused launch for the tail that reduces it (make_tail, launch_tail): the grid, the stride of the
+// partial vectors and the ReduceMap -- the p_net net-gradient entries, then the partial-vector entries of the two trained lambdas
+// (lam; nullptr when there are none) and of the data, boundary and residual loss parts.
+void record_launch(pinn_t* h, int grid, int stride, int p_net, const int* lam, int l_data, int l_bnd, int l_res) {
+  pinn::ReduceMap map{};
+  map.p_net = p_net;
+  if (lam) { map.extra_src[map.n_extra++] = lam[0]; map.extra_src[map.n_extra++] = lam[1]; }
+  for (int s : {l_data, l_bnd, l_res}) map.extra_src[map.n_extra++] = s;
+  map.n_out = map.p_net + map.n_extra;
+  h->last_map = map; h->last_grid = grid; h->last_stride = stride;
+}
+
 struct AdamArgs { double lr, b1, b2, eps; };
 
 // The tail of h's most recent fused launch (h->last_map): with Adam when ad != nullptr, with the P2P exchange when world > 1 and
@@ -433,14 +566,15 @@ bool tail_slot_free(pinn_t* h) {
 // its last CTAs (fused_tail); *tail_done tells the caller that no tail kernel is needed.  PINN_FUSED_TAIL=0 keeps the tail kernel.
 int burgers_launch_eval(pinn_t* h, const int* run_flag, const AdamArgs* ad = nullptr, bool* tail_done = nullptr) {
   namespace B = pinn::burgers;
-  const bool ide = h->pde == PINN_BURGERS_IDE;
+  const bool ide = model(h).residual == Res::Data;
+  const bool v2 = h->kernel == Kernel::BurgersV2;
   const long long n_total = ide ? h->n_d : h->n_d + h->n_c;
   if (n_total <= 0) return fail("no points set (pinn_set_collocation / pinn_set_data)");
   B::Args a{};
   a.w = h->d_w;
   a.x = h->d_x + (h->dcap - h->n_d); a.t = h->d_t + (h->dcap - h->n_d); a.utgt = h->d_u;
   a.xc = h->map_x; a.tc = h->map_t;
-  if (h->map_x && h->burgers_kernel != 2) return fail("zero-copy collocation needs the v2 Burgers kernel");
+  if (h->map_x && !v2) return fail("zero-copy collocation needs the v2 Burgers kernel");
   a.n_total = n_total;
   a.c0 = ide ? 0 : h->n_d;
   a.n_c = ide ? h->n_d : h->n_c;
@@ -458,27 +592,20 @@ int burgers_launch_eval(pinn_t* h, const int* run_flag, const AdamArgs* ad = nul
   a.chains = 4;
   const long long n_tiles = (n_total + B::TILE - 1) / B::TILE;
   const long long rounds = (n_total + B::ROUND - 1) / B::ROUND;
-  const long long units = h->burgers_kernel == 2 ? n_tiles : rounds;
+  const long long units = v2 ? n_tiles : rounds;
   int grid = (int)(units < h->n_cta ? units : h->n_cta);
-  pinn::ReduceMap map{};
-  map.p_net = B::P_NET;
-  map.n_extra = 0;
-  if (ide) { map.extra_src[map.n_extra++] = B::IDX_DL1; map.extra_src[map.n_extra++] = B::IDX_DL2; }
-  map.extra_src[map.n_extra++] = B::IDX_LD;
-  map.extra_src[map.n_extra++] = 3023;        // (boundary part: always 0 for Burgers)
-  map.extra_src[map.n_extra++] = B::IDX_LF;
-  map.n_out = map.p_net + map.n_extra;
-  h->last_map = map; h->last_grid = grid; h->last_stride = B::PSTRIDE;
+  const int lam[2] = {B::IDX_DL1, B::IDX_DL2};
+  record_launch(h, grid, B::PSTRIDE, B::P_NET, ide ? lam : nullptr, B::IDX_LD, 3023, B::IDX_LF);   // (3023: the boundary part, always 0)
   static const bool fused_tail_on = [] { const char* e = getenv("PINN_FUSED_TAIL"); return !(e && e[0] == '0'); }();
   // every evaluation of the v2 kernel carries its own tail: Adam steps (ad != nullptr) and plain evaluations (L-BFGS, loss/gradient
   // queries; a launch skipped through run_flag skips its tail with it, exactly like the stand-alone tail kernel)
-  if (tail_done && fused_tail_on && (h->world == 1 || h->p2p_ready) && h->burgers_kernel == 2 && grid <= h->n_sm && tail_slot_free(h)) {
+  if (tail_done && fused_tail_on && (h->world == 1 || h->p2p_ready) && v2 && grid <= h->n_sm && tail_slot_free(h)) {
     if (make_tail(h, ad, &a.tail)) return -1;
     a.tail.enabled = 1;
     h->tail_inflight = true;
     *tail_done = true;
   }
-  if (h->burgers_kernel == 2)
+  if (v2)
     pinn::burgers2::fused_loss_grad<<<grid, pinn::burgers2::THREADS, pinn::burgers2::SMEM_BYTES, h->stream>>>(a);
   else
     B::fused_loss_grad<<<grid, B::THREADS, B::SMEM_BYTES, h->stream>>>(a);
@@ -489,49 +616,29 @@ int burgers_launch_eval(pinn_t* h, const int* run_flag, const AdamArgs* ad = nul
 
 // one evaluation: the fused loss/gradient kernel of the handle's PDE, then (unless fused_only) the tail
 int launch_eval(pinn_t* h, const int* run_flag, bool fused_only = false, const AdamArgs* ad = nullptr) {
-  int rc;
+  int rc = 0;
   bool tail_done = false;
-  if (h->kernel_kind == 2) rc = generic_launch_eval(h, run_flag);
-  else if (h->kernel_kind == 3) rc = ns_launch_eval(h, run_flag);
-  else if (h->pde == PINN_BURGERS_INF || h->pde == PINN_BURGERS_IDE) rc = burgers_launch_eval(h, run_flag, ad, fused_only ? nullptr : &tail_done);
-  else rc = nls_launch_eval(h, run_flag);
+  switch (h->kernel) {
+    case Kernel::BurgersV2:
+    case Kernel::BurgersV1: rc = burgers_launch_eval(h, run_flag, ad, fused_only ? nullptr : &tail_done); break;
+    case Kernel::Schrodinger: rc = nls_launch_eval(h, run_flag); break;
+    case Kernel::Generic: rc = generic_launch_eval(h, run_flag); break;
+    case Kernel::NavierStokes: rc = ns_launch_eval(h, run_flag); break;
+  }
   if (rc) return -1;
   if (fused_only || tail_done) return 0;
   return launch_tail(h, run_flag, ad);
 }
 
-// DISC: data region = [x_0 data points | x_1 boundary points], right-aligned like every data block (t is unused).
-// AC: [x_0 | pad to even | lb, ub]: the periodic pair starts at an even index, so it never straddles a CTA.
-int disc_upload_points(pinn_t* h) {
-  const bool ac = h->pde == PINN_AC_DISC;
-  const long long n0p = ac ? (h->n_d + 1) & ~1LL : h->n_d;
-  const long long n_aux = ac ? (h->n_d > 0 ? n0p + 2 : 0) : h->n_d + h->n_b;
-  if (ensure_points(h, n_aux > h->n_aux ? n_aux : h->n_aux, 0)) return -1;
-  h->stage_x.assign(n_aux, 0.0); h->stage_t.assign(n_aux, 0.0);
-  for (long long i = 0; i < h->n_d; i++) h->stage_x[i] = h->h_x0[i];
-  if (ac && n_aux) {
-    for (long long i = h->n_d; i < n0p; i++) h->stage_x[i] = h->lb[0];    // inert alignment point
-    h->stage_x[n0p] = h->lb[0]; h->stage_x[n0p + 1] = h->ub[0];
-  }
-  for (long long i = 0; !ac && i < h->n_b; i++) h->stage_x[h->n_d + i] = h->h_tb[i];
-  if (n_aux) {
-    CUDA_TRY(cudaMemcpyAsync(h->d_x + h->dcap - n_aux, h->stage_x.data(), n_aux * 8, cudaMemcpyHostToDevice, h->stream));
-    CUDA_TRY(cudaMemcpyAsync(h->d_t + h->dcap - n_aux, h->stage_t.data(), n_aux * 8, cudaMemcpyHostToDevice, h->stream));
-    CUDA_TRY(cudaStreamSynchronize(h->stream));
-  }
-  h->n_aux = n_aux;
-  return 0;
-}
-
 int generic_launch_eval(pinn_t* h, const int* run_flag) {
   namespace G = pinn::generic;
-  const bool idd = is_ide_disc(h->pde);
-  const bool disc = is_disc(h->pde);
-  if (disc && (!h->d_irk || h->irk_q + (idd ? 0 : 1) != h->layers.back())) return fail("discrete-time model: call pinn_set_irk first");
-  const bool poly = is_poly(h->pde);
-  if (poly && h->poly.n == 0) return fail("polynomial residual model: call pinn_set_residual first (no residual is set)");
-  const bool nls = h->pde == PINN_NLS_INF, ide = h->pde == PINN_BURGERS_IDE || h->pde == PINN_POLY_IDE;
-  const long long n_total = disc ? h->n_aux : (nls ? h->n_aux + h->n_c : (ide ? h->n_d : h->n_d + h->n_c));
+  const Model& m = model(h);
+  if (m.irk && (!h->d_irk || h->irk_q + (m.out == Out::QPlus1 ? 1 : 0) != h->layers.back()))
+    return fail("discrete-time model: call pinn_set_irk first");
+  if (m.poly && h->poly.n == 0) return fail("polynomial residual model: call pinn_set_residual first (no residual is set)");
+  const bool ide = m.residual == Res::Data;
+  // the kernel's points: the block right-aligned in the data region, then the collocation set (n_c is 0 for models without one)
+  const long long n_total = h->n_aux + h->n_c;
   if (n_total <= 0) return fail("no points set (pinn_set_collocation / pinn_set_data)");
   const long long per = (n_total + h->n_cta - 1) / h->n_cta;
   // points per CTA: a multiple of 16 for large sets; small sets (the discrete-time models have ~250 points) are spread over as
@@ -545,22 +652,14 @@ int generic_launch_eval(pinn_t* h, const int* run_flag) {
   const int out_w = nd.dims[nd.n_layers];
   if (out_w > maxw) maxw = out_w;                 // the IRK head reuses the adjoint scratch for N, N-bar and 2(U_0 - u_0)
   const long long a_per = 4 * pts * maxw;
-  if (pts > h->g_pts) {
-    if (h->d_gH) cudaFree(h->d_gH);
-    if (h->d_gA) cudaFree(h->d_gA);
-    if (h->d_gS) cudaFree(h->d_gS);
-    h->d_gH = h->d_gA = h->d_gS = nullptr;
-    CUDA_TRY(cudaMalloc((void**)&h->d_gH, (size_t)h->n_cta * hsum * 8));          // sized for the largest grid (all CTAs)
-    CUDA_TRY(cudaMalloc((void**)&h->d_gA, (size_t)h->n_cta * 2 * a_per * 8));
-    CUDA_TRY(cudaMalloc((void**)&h->d_gS, (size_t)h->n_cta * 2 * pts * 4 * out_w * 8));
-    h->g_pts = pts;
-  }
+  // sized for the largest grid (all CTAs)
+  if (h->scratch.reserve(pts, (size_t)h->n_cta * hsum * 8, (size_t)h->n_cta * 2 * a_per * 8, (size_t)h->n_cta * 2 * pts * 4 * out_w * 8))
+    return -1;
   G::Args a{};
   a.w = h->d_w; a.nd = nd;
-  const long long n_front = (nls || disc) ? h->n_aux : h->n_d;
-  a.x = h->d_x + (h->dcap - n_front); a.t = h->d_t + (h->dcap - n_front); a.tgt = h->d_u;
+  a.x = h->d_x + (h->dcap - h->n_aux); a.t = h->d_t + (h->dcap - h->n_aux); a.tgt = h->d_u;
   a.n_total = n_total; a.pde = h->pde;
-  a.in_dim = disc ? 1 : 2; a.dt = h->dt; a.irk = h->d_irk;
+  a.in_dim = m.in_dim; a.dt = h->dt; a.irk = h->d_irk;
   a.o3 = h->pde == PINN_KDV_IDE_DISC ? 1 : 0; a.kc = h->kc;
   a.c0 = ide ? 0 : h->n_d; a.n_c = ide ? h->n_d : h->n_c; a.d0 = 0; a.n_d = h->n_d;
   const long long nfg = ide ? h->n_d : h->n_c_global;
@@ -570,15 +669,15 @@ int generic_launch_eval(pinn_t* h, const int* run_flag) {
   a.n0 = h->n_d; a.n0p = (h->n_d + 1) & ~1LL; a.nb = h->n_b;
   a.w0 = h->n_d > 0 ? h->data_weight / (double)h->n_d : 0.0;
   a.wb = h->n_b > 0 ? h->data_weight / (double)h->n_b : 0.0;
-  if (nls && h->n_aux != a.n0p + 2 * a.nb) return fail("internal: NLS auxiliary block out of date");
+  if (h->pde == PINN_NLS_INF && h->n_aux != a.n0p + 2 * a.nb) return fail("internal: NLS auxiliary block out of date");
   a.p_net = h->P_net;
-  a.scrH = h->d_gH; a.scrA = h->d_gA; a.scrS = h->d_gS;
+  a.scrH = h->scratch.H; a.scrA = h->scratch.A; a.scrS = h->scratch.S;
   a.h_per_cta = hsum; a.a_per_cta = a_per;
   a.pts = (int)pts; a.maxw = maxw;
   static const bool generic_dfma = [] { const char* e = getenv("PINN_GENERIC_DFMA"); return e && e[0] == '1'; }();
   a.dmma = generic_dfma ? 0 : 1;
   a.partials = h->d_partials; a.pstride = h->pstride; a.run_flag = run_flag;
-  if (poly) {
+  if (m.poly) {
     a.poly = h->poly;
     a.src = h->h_src.empty() ? nullptr : h->d_src;
     G::fused_loss_grad<true><<<grid, G::THREADS, 0, h->stream>>>(a);
@@ -587,15 +686,8 @@ int generic_launch_eval(pinn_t* h, const int* run_flag) {
   }
   CUDA_TRY(cudaGetLastError());
   h->launches++;
-  pinn::ReduceMap map{};
-  map.p_net = h->P_net;
-  map.n_extra = 0;
-  if (ide || idd) { map.extra_src[map.n_extra++] = h->P_net + 0; map.extra_src[map.n_extra++] = h->P_net + 1; }
-  map.extra_src[map.n_extra++] = h->P_net + 3;
-  map.extra_src[map.n_extra++] = h->P_net + 4;
-  map.extra_src[map.n_extra++] = h->P_net + 5;
-  map.n_out = map.p_net + map.n_extra;
-  h->last_map = map; h->last_grid = grid; h->last_stride = h->pstride;
+  const int lam[2] = {h->P_net, h->P_net + 1};
+  record_launch(h, grid, h->pstride, h->P_net, m.n_lambda ? lam : nullptr, h->P_net + 3, h->P_net + 4, h->P_net + 5);
   return 0;
 }
 
@@ -611,32 +703,20 @@ int ns_launch_eval(pinn_t* h, const int* run_flag) {
   int maxw = 0; long long hsum = 0;
   for (int l = 0; l < nd.n_layers - 1; l++) { hsum += S::NST * pts * nd.dims[l + 1]; if (nd.dims[l + 1] > maxw) maxw = nd.dims[l + 1]; }
   const long long a_per = S::NST * pts * maxw;
-  if (pts > h->g_pts) {
-    if (h->d_gH) cudaFree(h->d_gH);
-    if (h->d_gA) cudaFree(h->d_gA);
-    if (h->d_gS) cudaFree(h->d_gS);
-    h->d_gH = h->d_gA = h->d_gS = nullptr;
-    CUDA_TRY(cudaMalloc((void**)&h->d_gH, (size_t)h->n_cta * hsum * 8));
-    CUDA_TRY(cudaMalloc((void**)&h->d_gA, (size_t)h->n_cta * 2 * a_per * 8));
-    CUDA_TRY(cudaMalloc((void**)&h->d_gS, (size_t)h->n_cta * 2 * pts * S::SEEDW * 8));
-    h->g_pts = pts;
-  }
+  if (h->scratch.reserve(pts, (size_t)h->n_cta * hsum * 8, (size_t)h->n_cta * 2 * a_per * 8, (size_t)h->n_cta * 2 * pts * S::SEEDW * 8))
+    return -1;
   S::Args a{};
   a.w = h->d_w; a.nd = nd;
   for (int c = 0; c < 3; c++) { a.lb[c] = h->lb[c]; a.sc[c] = 2.0 / (h->ub[c] - h->lb[c]); }
   a.X = h->d_nsX; a.tgt = h->d_u; a.n_total = n_total; a.p_net = h->P_net;
-  a.scrH = h->d_gH; a.scrA = h->d_gA; a.scrS = h->d_gS;
+  a.scrH = h->scratch.H; a.scrA = h->scratch.A; a.scrS = h->scratch.S;
   a.h_per_cta = hsum; a.a_per_cta = a_per; a.pts = (int)pts;
   a.partials = h->d_partials; a.pstride = h->pstride; a.run_flag = run_flag;
   S::fused_loss_grad<<<grid, S::THREADS, 0, h->stream>>>(a);
   CUDA_TRY(cudaGetLastError());
   h->launches++;
-  pinn::ReduceMap map{};
-  map.p_net = h->P_net;
-  map.n_extra = 5;
-  for (int k = 0; k < 5; k++) map.extra_src[k] = h->P_net + k;
-  map.n_out = map.p_net + map.n_extra;
-  h->last_map = map; h->last_grid = grid; h->last_stride = h->pstride;
+  const int lam[2] = {h->P_net, h->P_net + 1};
+  record_launch(h, grid, h->pstride, h->P_net, lam, h->P_net + 2, h->P_net + 3, h->P_net + 4);
   return 0;
 }
 
@@ -666,30 +746,6 @@ int ns_probe(pinn_t* h, const double* dX, int64_t n, int mode, double* out_host)
   return 0;
 }
 
-// NLS: (re)assemble the auxiliary block [initial-condition points | pad to even | (lb_k, ub_k) pairs] right-aligned in
-// the data region (inf_cont_schrodinger.py:50-53 builds X_lb=(0*tb+lb0,tb), X_ub=(0*tb+ub0,tb)).
-int nls_upload_points(pinn_t* h) {
-  const long long n0 = h->n_d, n0p = (n0 + 1) & ~1LL, nb = h->n_b;
-  const long long n_aux = n0p + 2 * nb;
-  // the right-aligned start moves with n_aux: grow first with the OLD count so nothing is lost, then rewrite
-  if (ensure_points(h, n_aux > h->n_aux ? n_aux : h->n_aux, h->n_c)) return -1;
-  h->stage_x.assign(n_aux, 0.0); h->stage_t.assign(n_aux, 0.0);
-  for (long long i = 0; i < n0; i++) { h->stage_x[i] = h->h_icx[i]; h->stage_t[i] = h->h_ict[i]; }
-  if (n0p > n0) { h->stage_x[n0] = h->lb[0]; h->stage_t[n0] = h->lb[1]; }     // inert alignment point
-  for (long long k = 0; k < nb; k++) {
-    // x as the reference forms it, 0 * tb + lb0: NaN for an infinite or NaN tb, lb0 (ub0) for every finite one
-    h->stage_x[n0p + 2 * k] = 0.0 * h->h_tb[k] + h->lb[0];     h->stage_t[n0p + 2 * k] = h->h_tb[k];
-    h->stage_x[n0p + 2 * k + 1] = 0.0 * h->h_tb[k] + h->ub[0]; h->stage_t[n0p + 2 * k + 1] = h->h_tb[k];
-  }
-  if (n_aux) {
-    CUDA_TRY(cudaMemcpyAsync(h->d_x + h->dcap - n_aux, h->stage_x.data(), n_aux * 8, cudaMemcpyHostToDevice, h->stream));
-    CUDA_TRY(cudaMemcpyAsync(h->d_t + h->dcap - n_aux, h->stage_t.data(), n_aux * 8, cudaMemcpyHostToDevice, h->stream));
-    CUDA_TRY(cudaStreamSynchronize(h->stream));
-  }
-  h->n_aux = n_aux;
-  return 0;
-}
-
 int nls_launch_eval(pinn_t* h, const int* run_flag) {
   namespace N = pinn::nls;
   const long long n0 = h->n_d, n0p = (n0 + 1) & ~1LL, nb = h->n_b;
@@ -699,16 +755,8 @@ int nls_launch_eval(pinn_t* h, const int* run_flag) {
   const int grid = h->n_cta;
   long long per = (n_total + grid - 1) / grid;
   const int pts = (int)((per + N::RPTS - 1) / N::RPTS * N::RPTS);
-  if (pts > h->scr_pts) {
-    if (h->d_scrH) cudaFree(h->d_scrH);
-    if (h->d_scrA) cudaFree(h->d_scrA);
-    if (h->d_scrS) cudaFree(h->d_scrS);
-    h->d_scrH = h->d_scrA = h->d_scrS = nullptr;
-    CUDA_TRY(cudaMalloc((void**)&h->d_scrH, (size_t)grid * 16 * pts * N::W * 8));
-    CUDA_TRY(cudaMalloc((void**)&h->d_scrA, (size_t)grid * 8 * pts * N::W * 8));
-    CUDA_TRY(cudaMalloc((void**)&h->d_scrS, (size_t)grid * pts * 8 * 8));
-    h->scr_pts = pts;
-  }
+  if (h->scratch.reserve(pts, (size_t)grid * 16 * pts * N::W * 8, (size_t)grid * 8 * pts * N::W * 8, (size_t)grid * pts * 8 * 8))
+    return -1;
   N::Args a{};
   a.w = h->d_w;
   a.x = h->d_x + (h->dcap - h->n_aux); a.t = h->d_t + (h->dcap - h->n_aux); a.uv0 = h->d_u;
@@ -717,20 +765,14 @@ int nls_launch_eval(pinn_t* h, const int* run_flag) {
   a.wb = nb > 0 ? h->data_weight / (double)nb : 0.0;
   a.wf = h->n_c_global > 0 ? 1.0 / (double)h->n_c_global : 0.0;
   a.lb0 = h->lb[0]; a.lb1 = h->lb[1]; a.dx0 = h->ub[0] - h->lb[0]; a.dx1 = h->ub[1] - h->lb[1];
-  a.scratchH = h->d_scrH; a.scratchA = h->d_scrA; a.scratchS = h->d_scrS;
-  a.pts = h->scr_pts;
+  a.scratchH = h->scratch.H; a.scratchA = h->scratch.A; a.scratchS = h->scratch.S;
   // the kernel derives its point range from a.pts, so keep the distribution even when the scratch is larger
   a.pts = pts;
   a.partials = h->d_partials; a.run_flag = run_flag;
   N::fused_loss_grad<<<grid, N::THREADS, N::SMEM_BYTES, h->stream>>>(a);
   CUDA_TRY(cudaGetLastError());
   h->launches++;
-  pinn::ReduceMap map{};
-  map.p_net = N::P_NET;
-  map.n_extra = 3;
-  map.extra_src[0] = N::IDX_L0; map.extra_src[1] = N::IDX_LB; map.extra_src[2] = N::IDX_LF;
-  map.n_out = map.p_net + map.n_extra;
-  h->last_map = map; h->last_grid = grid; h->last_stride = N::PSTRIDE;
+  record_launch(h, grid, N::PSTRIDE, N::P_NET, nullptr, N::IDX_L0, N::IDX_LB, N::IDX_LF);
   return 0;
 }
 
@@ -814,70 +856,54 @@ int pinn_create(pinn_t** out, int pde_id, int n_layers, const int* layers, const
   if (!out || !layers || !lb || !ub) return fail("pinn_create: null argument");
   if (n_layers < 3 || n_layers > pinn::MAXL) return fail("pinn_create: need 3..16 layer sizes");
   if (pde_id < 0 || pde_id > 9) return fail("pinn_create: unknown pde_id");
-  const bool ns = pde_id == PINN_NS_IDE;
-  if (ns && world > 1) return fail("pinn_create: the Navier-Stokes identification model runs on one GPU (world must be 1)");
-  // Sharding (utils/sharding.py) splits the collocation rows with the global 1/N_f and weights the replicated terms by the data
-  // weight.  The discrete-time heads have no collocation set and sum every term without a data weight, and Burgers
-  // identification puts its residual on the data points with the local 1/n_d: sharded, each of them counts the wrong loss.
-  if (world > 1 && (pde_id == PINN_BURGERS_IDE || is_disc(pde_id)))
-    return fail(pde_id == PINN_BURGERS_IDE
-                    ? "pinn_create: the Burgers identification model runs on one GPU (world must be 1): its residual sits on the data "
-                      "points, which carry no data weight"
-                    : "pinn_create: the discrete-time models run on one GPU (world must be 1): they have no collocation set to shard "
-                      "and their heads read no data weight");
-  if (is_poly(pde_id)) {
-    if (world > 1) return fail("pinn_create: the polynomial residual models run on one GPU (world must be 1)");
-    if (layers[0] != 2 || layers[n_layers - 1] != 1)
-      return fail("pinn_create: unknown pde_id for a [" + std::to_string(layers[0]) + ", ..., " + std::to_string(layers[n_layers - 1]) +
-                  "] net: the polynomial residual models (8, 9) take a net [2, ..., 1]: (x, t) -> u");
-  }
+  const Model& m = MODELS[pde_id];
+  if (world > 1 && m.no_shard) return fail(m.no_shard);
+  const int q = layers[n_layers - 1];
+  if (m.poly && (layers[0] != 2 || q != 1))
+    return fail("pinn_create: unknown pde_id for a [" + std::to_string(layers[0]) + ", ..., " + std::to_string(q) +
+                "] net: the polynomial residual models (8, 9) take a net [2, ..., 1]: (x, t) -> u");
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
     return fail("pinn_create: no CUDA device -- this library has no CPU fallback");
   if (device < 0 || device >= ndev) return fail("pinn_create: bad device index");
+  for (int i = 0; i < n_layers; i++)
+    if (layers[i] < 1 || layers[i] > (i == n_layers - 1 ? m.head_cap : pinn::MAXW_WIDE))
+      return fail("pinn_create: layer width out of range (1..256; IRK head <= 512)");
+  if (m.in_dim == 3 ? (layers[0] != 3 || q != 2) : layers[0] != m.in_dim)
+    return fail(m.in_dim == 3   ? "pinn_create: the Navier-Stokes identification model needs a net [3, ..., 2]: (x, y, t) -> (psi, p)"
+                : m.in_dim == 1 ? "pinn_create: the discrete-time model takes a 1-D input (x)"
+                                : "pinn_create: input dimension must be 2 (x,t)");
+  double lo[3] = {0.0, 0.0, 0.0}, hi[3] = {1.0, 1.0, 1.0};     // an axis the model does not have (t of a 1-D net) keeps [0, 1]
+  for (int c = 0; c < m.in_dim; c++) { lo[c] = lb[c]; hi[c] = ub[c]; }
+  if (!(hi[0] > lo[0]) || !(hi[1] > lo[1]) || !(hi[2] > lo[2])) return fail("pinn_create: need ub > lb");
+  switch (m.out) {
+    case Out::One: if (q != 1) return fail("pinn_create: the Burgers problems need 1 network output (u)"); break;
+    case Out::Two: if (q != 2) return fail("pinn_create: the Schrodinger problem needs 2 network outputs (u, v)"); break;
+    case Out::QPlus1: if (q < 2) return fail("pinn_create: the discrete-time model needs q+1 >= 2 outputs"); break;
+    case Out::Q: if (q < 1) return fail("pinn_create: the discrete-time identification model needs q >= 1 outputs"); break;
+  }
+  if (world > 1 && !nccl_uid) return fail("pinn_create: world > 1 needs an ncclUniqueId");
+
+  // the specialised DMMA kernels run their model's BASELINE net; any other layer list runs on the generic kernel
+  const std::vector<int> L(layers, layers + n_layers);
+  const char* fg = getenv("PINN_FORCE_GENERIC");
+  const bool force = fg && fg[0] == '1';
+  Kernel kernel = m.kernel;
+  if (kernel == Kernel::Schrodinger && (force || !is_nls_net(L))) kernel = Kernel::Generic;
+  if (kernel == Kernel::BurgersV2) {
+    const char* kv = getenv("PINN_BURGERS_KERNEL");
+    if (force || !is_burgers_net(L)) kernel = Kernel::Generic;
+    else if (kv && (!strcmp(kv, "v1") || !strcmp(kv, "1"))) kernel = Kernel::BurgersV1;
+  }
+
   pinn_t* h = new pinn_t();
   h->pde = pde_id; h->device = device; h->rank = rank; h->world = world < 1 ? 1 : world;
-  h->layers.assign(layers, layers + n_layers);
-  const bool disc = is_disc(pde_id);
-  for (int i = 0; i < n_layers; i++) {
-    const int v = h->layers[i];
-    const int cap = (disc && i == n_layers - 1) ? 512 : pinn::MAXW_WIDE;     // the IRK head may be q+1 = 501 wide
-    if (v < 1 || v > cap) { delete h; return fail("pinn_create: layer width out of range (1..256; IRK head <= 512)"); }
-  }
-  if (ns) {
-    if (h->layers[0] != 3 || h->layers.back() != 2) {
-      delete h;
-      return fail("pinn_create: the Navier-Stokes identification model needs a net [3, ..., 2]: (x, y, t) -> (psi, p)");
-    }
-  } else if (h->layers[0] != (disc ? 1 : 2)) {
-    delete h;
-    return fail(disc ? "pinn_create: the discrete-time model takes a 1-D input (x)" : "pinn_create: input dimension must be 2 (x,t)");
-  }
-  h->lb[0] = lb[0]; h->ub[0] = ub[0];
-  h->lb[1] = disc ? 0.0 : lb[1]; h->ub[1] = disc ? 1.0 : ub[1];            // the t axis does not exist for 1-D nets
-  if (ns) { h->lb[2] = lb[2]; h->ub[2] = ub[2]; }
-  if (!(h->ub[0] > h->lb[0]) || !(h->ub[1] > h->lb[1]) || !(h->ub[2] > h->lb[2])) { delete h; return fail("pinn_create: need ub > lb"); }
-  const int want_out = pde_id == PINN_NLS_INF ? 2 : 1;
-  if (ns) {
-  } else if (is_ide_disc(pde_id)) {
-    if (h->layers.back() < 1) { delete h; return fail("pinn_create: the discrete-time identification model needs q >= 1 outputs"); }
-  } else if (disc) {
-    if (h->layers.back() < 2) { delete h; return fail("pinn_create: the discrete-time model needs q+1 >= 2 outputs"); }
-  } else if (h->layers.back() != want_out) {
-    delete h;
-    return fail(pde_id == PINN_NLS_INF ? "pinn_create: the Schrodinger problem needs 2 network outputs (u, v)"
-                                        : "pinn_create: the Burgers problems need 1 network output (u)");
-  }
-  {
-    // specialised DMMA kernels for the two BASELINE nets, generic DFMA kernel for any other layer list
-    const char* fg = getenv("PINN_FORCE_GENERIC");
-    const bool force = fg && fg[0] == '1';
-    const bool special = (disc || is_poly(pde_id)) ? false : ((pde_id == PINN_NLS_INF) ? is_nls_net(h->layers) : is_burgers_net(h->layers));
-    h->kernel_kind = ns ? 3 : (special && !force) ? (pde_id == PINN_NLS_INF ? 1 : 0) : 2;
-  }
+  h->layers = L;
+  for (int c = 0; c < 3; c++) { h->lb[c] = lo[c]; h->ub[c] = hi[c]; }
+  h->kernel = kernel;
   h->P_net = 0;
   for (int l = 0; l + 1 < n_layers; l++) h->P_net += layers[l] * layers[l + 1] + layers[l + 1];
-  h->P = h->P_net + ((pde_id == PINN_BURGERS_IDE || is_ide_disc(pde_id) || ns || pde_id == PINN_POLY_IDE) ? 2 : 0);
+  h->P = h->P_net + m.n_lambda;
 
 #define CREATE_TRY(expr)                                                                          \
   do {                                                                                            \
@@ -915,29 +941,32 @@ int pinn_create(pinn_t** out, int pde_id, int n_layers, const int* layers, const
   CREATE_TRY(cudaMemset(h->d_step, 0, 16));
   CREATE_TRY(cudaMalloc((void**)&h->d_loss_ring, LOSS_RING * 8));
   CREATE_TRY(cudaMemset(h->d_loss_ring, 0, LOSS_RING * 8));
-  if (h->kernel_kind == 3) {
-    h->n_cta = h->n_sm;
-    h->pstride = ((h->P_net + 8 + 15) / 16) * 16;
-  } else if (h->kernel_kind == 2) {
-    h->n_cta = 2 * h->n_sm;
-    h->pstride = ((h->P_net + 8 + 15) / 16) * 16;
-  } else if (pde_id == PINN_NLS_INF) {
-    h->n_cta = pinn::nls::grid_size(h->n_sm);
-    h->pstride = pinn::nls::PSTRIDE;
-    CREATE_TRY(cudaFuncSetAttribute(pinn::nls::fused_loss_grad, cudaFuncAttributeMaxDynamicSharedMemorySize, pinn::nls::SMEM_BYTES));
-  } else {
-    h->n_cta = h->n_sm;
-    h->pstride = pinn::burgers::PSTRIDE;
-    CREATE_TRY(cudaFuncSetAttribute(pinn::burgers::fused_loss_grad, cudaFuncAttributeMaxDynamicSharedMemorySize, pinn::burgers::SMEM_BYTES));
-    CREATE_TRY(cudaFuncSetAttribute(pinn::burgers2::fused_loss_grad, cudaFuncAttributeMaxDynamicSharedMemorySize, pinn::burgers2::SMEM_BYTES));
-    const char* kv = getenv("PINN_BURGERS_KERNEL");
-    if (kv && (!strcmp(kv, "v1") || !strcmp(kv, "1"))) h->burgers_kernel = 1;
+  switch (h->kernel) {
+    case Kernel::BurgersV2:
+      h->n_cta = h->n_sm;
+      h->pstride = pinn::burgers::PSTRIDE;
+      CREATE_TRY(cudaFuncSetAttribute(pinn::burgers2::fused_loss_grad, cudaFuncAttributeMaxDynamicSharedMemorySize, pinn::burgers2::SMEM_BYTES));
+      break;
+    case Kernel::BurgersV1:
+      h->n_cta = h->n_sm;
+      h->pstride = pinn::burgers::PSTRIDE;
+      CREATE_TRY(cudaFuncSetAttribute(pinn::burgers::fused_loss_grad, cudaFuncAttributeMaxDynamicSharedMemorySize, pinn::burgers::SMEM_BYTES));
+      break;
+    case Kernel::Schrodinger:
+      h->n_cta = pinn::nls::grid_size(h->n_sm);
+      h->pstride = pinn::nls::PSTRIDE;
+      CREATE_TRY(cudaFuncSetAttribute(pinn::nls::fused_loss_grad, cudaFuncAttributeMaxDynamicSharedMemorySize, pinn::nls::SMEM_BYTES));
+      break;
+    case Kernel::Generic:
+    case Kernel::NavierStokes:
+      h->n_cta = (h->kernel == Kernel::Generic ? 2 : 1) * h->n_sm;     // CTAs of 256 threads: two per SM, or one (Navier-Stokes)
+      h->pstride = ((h->P_net + 8 + 15) / 16) * 16;
+      break;
   }
   CREATE_TRY(cudaMalloc((void**)&h->d_partials, (size_t)h->n_cta * h->pstride * 8));
   CREATE_TRY(cudaMemset(h->d_partials, 0, (size_t)h->n_cta * h->pstride * 8));
   if (h->world > 1) {
     std::string why;
-    if (!nccl_uid) { fail("pinn_create: world > 1 needs an ncclUniqueId"); pinn_destroy(h); return -1; }
     if (!g_nccl.load(why)) { fail(why); pinn_destroy(h); return -1; }
     ncclUniqueId id;
     memcpy(&id, nccl_uid, 128);
@@ -963,10 +992,11 @@ int pinn_destroy(pinn_t* h) {
   if (h->d_p2p_err) cudaFree(h->d_p2p_err);
   if (h->d_xseq) cudaFree(h->d_xseq);
   if (h->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(h->comm);
-  double* bufs[] = {h->d_w, h->d_R, h->d_partials, h->d_m, h->d_v, h->d_loss_ring, h->d_x, h->d_t, h->d_u, h->d_scrH, h->d_scrA, h->d_scrS, h->d_gH, h->d_gA, h->d_gS, h->d_irk,
+  double* bufs[] = {h->d_w, h->d_R, h->d_partials, h->d_m, h->d_v, h->d_loss_ring, h->d_x, h->d_t, h->d_u, h->d_irk,
                     h->d_px, h->d_pout, h->d_pscr, h->d_nsX, h->d_src};
   for (double* b : bufs) if (b) cudaFree(b);
   if (h->d_step) cudaFree(h->d_step);
+  h->scratch.release();
   h->lbfgs.release();
   for (cudaEvent_t e : h->events) cudaEventDestroy(e);
   if (h->d_flush) cudaFree(h->d_flush);
@@ -981,25 +1011,24 @@ int64_t pinn_num_params(const pinn_t* h) { return h ? h->P : -1; }
 
 int pinn_set_pde_params(pinn_t* h, const double* p, int n) {
   if (!h) return fail("null handle");
-  if (h->pde == PINN_BURGERS_INF) {
-    if (n != 1 || !p) return fail("pinn_set_pde_params: BURGERS_INF takes exactly one parameter (nu)");
-    h->nu = p[0];
-    return 0;
-  }
-  if (h->pde == PINN_BURGERS_DISC) {
-    if (n != 2 || !p) return fail("pinn_set_pde_params: BURGERS_DISC takes [nu, dt]");
-    h->nu = p[0]; h->dt = p[1];
-    return 0;
-  }
-  if (is_ide_disc(h->pde)) {
-    if (n != 1 || !p) return fail("pinn_set_pde_params: the discrete-time identification models take [dt]");
-    h->dt = p[0];
-    return 0;
-  }
-  if (h->pde == PINN_AC_DISC) {
-    if (n != 3 || !p) return fail("pinn_set_pde_params: AC_DISC takes [dt, d, k]");
-    h->dt = p[0]; h->nu = p[1]; h->kc = p[2];
-    return 0;
+  switch (h->pde) {
+    case PINN_BURGERS_INF:
+      if (n != 1 || !p) return fail("pinn_set_pde_params: BURGERS_INF takes exactly one parameter (nu)");
+      h->nu = p[0];
+      return 0;
+    case PINN_BURGERS_DISC:
+      if (n != 2 || !p) return fail("pinn_set_pde_params: BURGERS_DISC takes [nu, dt]");
+      h->nu = p[0]; h->dt = p[1];
+      return 0;
+    case PINN_BURGERS_IDE_DISC:
+    case PINN_KDV_IDE_DISC:
+      if (n != 1 || !p) return fail("pinn_set_pde_params: the discrete-time identification models take [dt]");
+      h->dt = p[0];
+      return 0;
+    case PINN_AC_DISC:
+      if (n != 3 || !p) return fail("pinn_set_pde_params: AC_DISC takes [dt, d, k]");
+      h->dt = p[0]; h->nu = p[1]; h->kc = p[2];
+      return 0;
   }
   if (n != 0) return fail("pinn_set_pde_params: this PDE takes no constants");
   return 0;
@@ -1007,37 +1036,38 @@ int pinn_set_pde_params(pinn_t* h, const double* p, int n) {
 
 int pinn_get_params(pinn_t* h, double* p, int n) {
   if (!h || !p) return fail("pinn_get_params: null argument");
-  if (h->pde == PINN_BURGERS_INF) {
-    if (n != 1) return fail("pinn_get_params: BURGERS_INF has one parameter (nu)");
-    p[0] = h->nu;                                   // inf_cont_burgers.py:92-93
-    return 0;
-  }
-  if (h->pde == PINN_BURGERS_IDE || is_ide_disc(h->pde)) {
-    if (n != 2) return fail("pinn_get_params: identification has two parameters (lambda_1, exp(lambda_2))");
-    CUDA_TRY(cudaSetDevice(h->device));
-    double lam[2];
-    CUDA_TRY(cudaMemcpyAsync(lam, h->d_w + h->P_net, 16, cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(cudaStreamSynchronize(h->stream));
-    p[0] = lam[0]; p[1] = std::exp(lam[1]);         // ide_cont_burgers.py:109-114, ide_disc_burgers.py:138-143
-    return 0;
-  }
-  if (h->pde == PINN_NS_IDE || h->pde == PINN_POLY_IDE) {
-    if (n != 2) return fail(h->pde == PINN_NS_IDE ? "pinn_get_params: NS_IDE has two parameters (lambda_1, lambda_2)"
-                                                  : "pinn_get_params: POLY_IDE has two parameters (the raw lambda_1, lambda_2)");
-    CUDA_TRY(cudaSetDevice(h->device));
-    CUDA_TRY(cudaMemcpyAsync(p, h->d_w + h->P_net, 16, cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(cudaStreamSynchronize(h->stream));
-    return 0;
-  }
-  if (h->pde == PINN_BURGERS_DISC) {
-    if (n != 2) return fail("pinn_get_params: BURGERS_DISC has two constants (nu, dt)");
-    p[0] = h->nu; p[1] = h->dt;
-    return 0;
-  }
-  if (h->pde == PINN_AC_DISC) {
-    if (n != 3) return fail("pinn_get_params: AC_DISC has three constants (dt, d, k)");
-    p[0] = h->dt; p[1] = h->nu; p[2] = h->kc;
-    return 0;
+  switch (h->pde) {
+    case PINN_BURGERS_INF:
+      if (n != 1) return fail("pinn_get_params: BURGERS_INF has one parameter (nu)");
+      p[0] = h->nu;                                   // inf_cont_burgers.py:92-93
+      return 0;
+    case PINN_BURGERS_IDE:
+    case PINN_BURGERS_IDE_DISC:
+    case PINN_KDV_IDE_DISC: {
+      if (n != 2) return fail("pinn_get_params: identification has two parameters (lambda_1, exp(lambda_2))");
+      CUDA_TRY(cudaSetDevice(h->device));
+      double lam[2];
+      CUDA_TRY(cudaMemcpyAsync(lam, h->d_w + h->P_net, 16, cudaMemcpyDeviceToHost, h->stream));
+      CUDA_TRY(cudaStreamSynchronize(h->stream));
+      p[0] = lam[0]; p[1] = std::exp(lam[1]);         // ide_cont_burgers.py:109-114, ide_disc_burgers.py:138-143
+      return 0;
+    }
+    case PINN_NS_IDE:
+    case PINN_POLY_IDE:
+      if (n != 2) return fail(h->pde == PINN_NS_IDE ? "pinn_get_params: NS_IDE has two parameters (lambda_1, lambda_2)"
+                                                    : "pinn_get_params: POLY_IDE has two parameters (the raw lambda_1, lambda_2)");
+      CUDA_TRY(cudaSetDevice(h->device));
+      CUDA_TRY(cudaMemcpyAsync(p, h->d_w + h->P_net, 16, cudaMemcpyDeviceToHost, h->stream));
+      CUDA_TRY(cudaStreamSynchronize(h->stream));
+      return 0;
+    case PINN_BURGERS_DISC:
+      if (n != 2) return fail("pinn_get_params: BURGERS_DISC has two constants (nu, dt)");
+      p[0] = h->nu; p[1] = h->dt;
+      return 0;
+    case PINN_AC_DISC:
+      if (n != 3) return fail("pinn_get_params: AC_DISC has three constants (dt, d, k)");
+      p[0] = h->dt; p[1] = h->nu; p[2] = h->kc;
+      return 0;
   }
   if (n != 0) return fail("pinn_get_params: this PDE has no parameters");
   return 0;
@@ -1045,8 +1075,8 @@ int pinn_get_params(pinn_t* h, double* p, int n) {
 
 int pinn_set_irk(pinn_t* h, const double* irk, int q) {
   if (!h || !irk) return fail("pinn_set_irk: null argument");
-  if (!is_disc(h->pde)) return fail("pinn_set_irk: only the discrete-time models have stage matrices");
-  const bool idd = is_ide_disc(h->pde);
+  if (!model(h).irk) return fail("pinn_set_irk: only the discrete-time models have stage matrices");
+  const bool idd = model(h).out == Out::Q;                         // identification: a net [1, ..., q]
   if (!idd && q + 1 != h->layers.back()) return fail("pinn_set_irk: q+1 must equal the network's output width");
   if (idd && q != h->layers.back()) return fail("pinn_set_irk: q must equal the network's output width");
   const size_t n_rows = idd ? (size_t)2 * q : (size_t)q + 1;      // identification: [M_0 ; M_1], each q x q
@@ -1061,9 +1091,9 @@ int pinn_set_irk(pinn_t* h, const double* irk, int q) {
 
 int pinn_set_collocation(pinn_t* h, const double* x, const double* t, int64_t n, int64_t n_global) {
   if (!h) return fail("null handle");
-  if (residual_on_data(h->pde))
+  if (model(h).residual == Res::Data)
     return fail("pinn_set_collocation: identification uses the data points as residual points");
-  if (is_disc(h->pde))
+  if (model(h).residual == Res::None)
     return fail("pinn_set_collocation: the discrete-time models have no collocation set (snapshot / boundary points only)");
   if (n < 0 || (n > 0 && (!x || !t))) return fail("pinn_set_collocation: bad arguments");
   if (n_global < n) return fail("pinn_set_collocation: n_global < n");
@@ -1083,7 +1113,7 @@ int pinn_set_collocation(pinn_t* h, const double* x, const double* t, int64_t n,
 
 int pinn_set_collocation_mapped(pinn_t* h, const double* x_pinned, const double* t_pinned, int64_t n, int64_t n_global) {
   if (!h) return fail("null handle");
-  if (h->kernel_kind != 0 || h->pde != PINN_BURGERS_INF)
+  if ((h->kernel != Kernel::BurgersV2 && h->kernel != Kernel::BurgersV1) || model(h).residual != Res::Colloc)
     return fail("pinn_set_collocation_mapped: zero-copy collocation is implemented for the fused Burgers inference kernel only");
   if (n <= 0 || !x_pinned || !t_pinned || n_global < n) return fail("pinn_set_collocation_mapped: bad arguments");
   CUDA_TRY(cudaSetDevice(h->device));
@@ -1103,72 +1133,48 @@ int pinn_set_collocation_mapped(pinn_t* h, const double* x_pinned, const double*
 int pinn_set_data(pinn_t* h, const double* X, int64_t n, int in_dim, const double* u, int out_dim, double weight) {
   if (!h) return fail("null handle");
   if (n < 0 || (n > 0 && (!X || !u))) return fail("pinn_set_data: bad arguments");
-  if (h->pde == PINN_NS_IDE) {
+  const Model& m = model(h);
+  if (m.in_dim == 3) {
     // X (n,3) = (x, y, t), u (n,2) = (u, v); these points also carry the residual term
     if (in_dim != 3 || out_dim != 2) return fail("pinn_set_data: the Navier-Stokes model takes X (n,3) = (x, y, t) and u (n,2) = (u, v)");
     CUDA_TRY(cudaSetDevice(h->device));
-    if (n) {
-      if (ensure(&h->d_nsX, &h->nsx_cap, 3 * n) || ensure(&h->d_u, &h->u_cap, 2 * n)) return -1;
-      CUDA_TRY(cudaMemcpyAsync(h->d_nsX, X, n * 3 * 8, cudaMemcpyHostToDevice, h->stream));
-      CUDA_TRY(cudaMemcpyAsync(h->d_u, u, n * 2 * 8, cudaMemcpyHostToDevice, h->stream));
-      CUDA_TRY(cudaStreamSynchronize(h->stream));
-    }
+    if (upload(h, &h->d_nsX, &h->nsx_cap, X, 3 * n) || upload(h, &h->d_u, &h->u_cap, u, 2 * n)) return -1;
     h->n_d = n; h->d_out_dim = 2; h->data_weight = weight;
     return 0;
   }
   if (in_dim != 1 && in_dim != 2) return fail("pinn_set_data: in_dim must be 1 (broadcast quirk) or 2");
-  if (is_ide_disc(h->pde)) return pinn_set_snapshot(h, 0, X, n, u);
-  if (h->pde == PINN_BURGERS_DISC || h->pde == PINN_AC_DISC) {
+  if (m.snapshots) return pinn_set_snapshot(h, 0, X, n, u);
+  if (m.in_dim == 1) {
     // x_0 (n,1) and u_0 (n,1): the snapshot the q stages are fitted to (inf_disc_burgers.py:98-101; u_0 broadcasts)
     if (in_dim != 1 || out_dim != 1) return fail("pinn_set_data: the discrete-time model takes x_0 (n,1) and u_0 (n,1)");
     CUDA_TRY(cudaSetDevice(h->device));
     h->h_x0.assign(X, X + n);
-    if (n) {
-      if (ensure(&h->d_u, &h->u_cap, n)) return -1;
-      CUDA_TRY(cudaMemcpyAsync(h->d_u, u, n * 8, cudaMemcpyHostToDevice, h->stream));
-      CUDA_TRY(cudaStreamSynchronize(h->stream));
-    }
+    if (upload(h, &h->d_u, &h->u_cap, u, n)) return -1;
     h->n_d = n; h->d_out_dim = 1; h->data_weight = weight;
-    return disc_upload_points(h);
+    return assemble_points(h);
   }
   if (out_dim != h->layers.back()) return fail("pinn_set_data: out_dim does not match the network head");
   CUDA_TRY(cudaSetDevice(h->device));
-  if (h->pde == PINN_NLS_INF) {
-    h->h_icx.resize(n); h->h_ict.resize(n);
-    for (int64_t i = 0; i < n; i++) {
-      h->h_icx[i] = X[i * in_dim];
-      h->h_ict[i] = in_dim == 1 ? X[i] : X[i * in_dim + 1];   // quirk Q1: (N,1) input broadcast, t := x
-    }
-    if (n) {
-      if (ensure(&h->d_u, &h->u_cap, n * out_dim)) return -1;
-      CUDA_TRY(cudaMemcpyAsync(h->d_u, u, n * out_dim * 8, cudaMemcpyHostToDevice, h->stream));
-      CUDA_TRY(cudaStreamSynchronize(h->stream));
-    }
-    h->n_d = n; h->d_out_dim = out_dim; h->data_weight = weight;
-    return nls_upload_points(h);
-  }
-  // shrinking/growing the data set moves its right-aligned start; the collocation region is untouched
-  if (ensure_points(h, n, h->n_c)) return -1;
-  h->stage_x.resize(n); h->stage_t.resize(n);
+  // the Schrodinger block is re-assembled with the boundary pairs, so it keeps host copies; the others are staged directly
+  std::vector<double>& x = m.boundary ? h->h_icx : h->stage_x;
+  std::vector<double>& t = m.boundary ? h->h_ict : h->stage_t;
+  x.resize(n); t.resize(n);
   for (int64_t i = 0; i < n; i++) {
-    h->stage_x[i] = X[i * in_dim];
-    h->stage_t[i] = in_dim == 1 ? X[i] : X[i * in_dim + 1];   // (N,1) input broadcast by the Lambda: t := x
+    x[i] = X[i * in_dim];
+    t[i] = in_dim == 1 ? X[i] : X[i * in_dim + 1];   // quirk Q1: the (N,1) input is broadcast by the Lambda, t := x
   }
-  if (n) {
-    if (ensure(&h->d_u, &h->u_cap, n * out_dim)) return -1;
-    CUDA_TRY(cudaMemcpyAsync(h->d_x + h->dcap - n, h->stage_x.data(), n * 8, cudaMemcpyHostToDevice, h->stream));
-    CUDA_TRY(cudaMemcpyAsync(h->d_t + h->dcap - n, h->stage_t.data(), n * 8, cudaMemcpyHostToDevice, h->stream));
-    CUDA_TRY(cudaMemcpyAsync(h->d_u, u, n * out_dim * 8, cudaMemcpyHostToDevice, h->stream));
-    CUDA_TRY(cudaStreamSynchronize(h->stream));
-  }
-  h->n_d = n; h->n_aux = n; h->d_out_dim = out_dim; h->data_weight = weight;
-  if (h->pde == PINN_POLY_IDE) h->h_src.clear();  // new residual points: the source is 0 until set again
+  if (upload(h, &h->d_u, &h->u_cap, u, n * out_dim)) return -1;
+  h->n_d = n; h->d_out_dim = out_dim; h->data_weight = weight;
+  if (m.boundary) return assemble_points(h);
+  // shrinking/growing the data set moves its right-aligned start; the collocation region is untouched
+  if (upload_points(h)) return -1;
+  if (m.residual == Res::Data) h->h_src.clear();   // new residual points: the source is 0 until set again
   return 0;
 }
 
 int pinn_set_residual(pinn_t* h, int n_terms, const double* coef, const int* kind, const int* exps) {
   if (!h) return fail("null handle");
-  if (!is_poly(h->pde)) return fail("pinn_set_residual: only the polynomial residual models (POLY_INF, POLY_IDE) take a residual spec");
+  if (!model(h).poly) return fail("pinn_set_residual: only the polynomial residual models (POLY_INF, POLY_IDE) take a residual spec");
   if (n_terms < 1 || n_terms > pinn::generic::POLY_MAXT)
     return fail("pinn_set_residual: n_terms = " + std::to_string(n_terms) + " is outside 1..16");
   if (!coef || !kind || !exps) return fail("pinn_set_residual: null argument");
@@ -1178,7 +1184,7 @@ int pinn_set_residual(pinn_t* h, int n_terms, const double* coef, const int* kin
     const std::string term = "pinn_set_residual: term " + std::to_string(k) + ": ";
     if (!std::isfinite(coef[k])) return fail(term + "the coefficient is not finite");
     if (kind[k] < 0 || kind[k] > 4) return fail(term + "kind " + std::to_string(kind[k]) + " is outside 0..4 (1, l1, l2, e^l1, e^l2)");
-    if (kind[k] != 0 && h->pde == PINN_POLY_INF)
+    if (kind[k] != 0 && model(h).n_lambda == 0)
       return fail(term + "POLY_INF has no trainable lambdas: every kind must be 0 (use POLY_IDE for l1, l2, e^l1, e^l2)");
     int code = kind[k], any = 0;
     for (int j = 0; j < 4; j++) {
@@ -1197,25 +1203,21 @@ int pinn_set_residual(pinn_t* h, int n_terms, const double* coef, const int* kin
 
 int pinn_set_source(pinn_t* h, const double* src, int64_t n) {
   if (!h) return fail("null handle");
-  if (!is_poly(h->pde)) return fail("pinn_set_source: only the polynomial residual models (POLY_INF, POLY_IDE) take a source");
+  if (!model(h).poly) return fail("pinn_set_source: only the polynomial residual models (POLY_INF, POLY_IDE) take a source");
   const int64_t want = pinn_num_residual_points(h);
   if (n != want)
     return fail("pinn_set_source: " + std::to_string(n) + " values given but " + std::to_string(want) +
                 " residual points are stored (pinn_num_residual_points)");
   if (n > 0 && !src) return fail("pinn_set_source: null argument");
   CUDA_TRY(cudaSetDevice(h->device));
-  if (n > 0) {
-    if (ensure(&h->d_src, &h->src_cap, n)) return -1;
-    CUDA_TRY(cudaMemcpyAsync(h->d_src, src, n * 8, cudaMemcpyHostToDevice, h->stream));
-    CUDA_TRY(cudaStreamSynchronize(h->stream));
-  }
+  if (upload(h, &h->d_src, &h->src_cap, src, n)) return -1;
   h->h_src.assign(src, src + n);
   return 0;
 }
 
 int pinn_set_snapshot(pinn_t* h, int which, const double* x, int64_t n, const double* u) {
   if (!h) return fail("null handle");
-  if (!is_ide_disc(h->pde)) return fail("pinn_set_snapshot: only the discrete-time identification models have two snapshots");
+  if (!model(h).snapshots) return fail("pinn_set_snapshot: only the discrete-time identification models have two snapshots");
   if ((which != 0 && which != 1) || n < 0 || (n > 0 && (!x || !u))) return fail("pinn_set_snapshot: bad arguments");
   CUDA_TRY(cudaSetDevice(h->device));
   // host copies of both snapshots: the device blocks [x_0 | x_1] and [u_0 | u_1] are re-assembled whenever one changes
@@ -1224,32 +1226,21 @@ int pinn_set_snapshot(pinn_t* h, int which, const double* x, int64_t n, const do
   h->n_d = (long long)h->h_x0.size();
   h->n_b = (long long)h->h_tb.size();
   h->d_out_dim = 1; h->data_weight = 1.0;
-  const long long nu = h->n_d + h->n_b;
-  if (nu) {
-    if (ensure(&h->d_u, &h->u_cap, nu)) return -1;
-    if (h->n_d) CUDA_TRY(cudaMemcpyAsync(h->d_u, h->h_u0.data(), h->n_d * 8, cudaMemcpyHostToDevice, h->stream));
-    if (h->n_b) CUDA_TRY(cudaMemcpyAsync(h->d_u + h->n_d, h->h_u1.data(), h->n_b * 8, cudaMemcpyHostToDevice, h->stream));
-    CUDA_TRY(cudaStreamSynchronize(h->stream));
-  }
-  return disc_upload_points(h);
+  std::vector<double> u01(h->h_u0);
+  u01.insert(u01.end(), h->h_u1.begin(), h->h_u1.end());
+  if (upload(h, &h->d_u, &h->u_cap, u01.data(), (long long)u01.size())) return -1;
+  return assemble_points(h);
 }
 
 int pinn_set_boundary(pinn_t* h, const double* tb, int64_t n_b) {
   if (!h) return fail("null handle");
-  if (h->pde == PINN_BURGERS_DISC) {
-    if (n_b < 0 || (n_b > 0 && !tb)) return fail("pinn_set_boundary: bad arguments");
-    h->h_tb.assign(tb, tb + n_b);
-    h->n_b = n_b;
-    CUDA_TRY(cudaSetDevice(h->device));
-    return disc_upload_points(h);
-  }
   if (h->pde == PINN_AC_DISC) return fail("pinn_set_boundary: the Allen-Cahn model's periodic pair is (lb, ub) of pinn_create");
-  if (h->pde != PINN_NLS_INF) return fail("pinn_set_boundary: only the NLS and discrete-time inference problems have a boundary term");
+  if (!model(h).boundary) return fail("pinn_set_boundary: only the NLS and discrete-time inference problems have a boundary term");
   if (n_b < 0 || (n_b > 0 && !tb)) return fail("pinn_set_boundary: bad arguments");
   h->h_tb.assign(tb, tb + n_b);
   h->n_b = n_b;
   CUDA_TRY(cudaSetDevice(h->device));
-  return nls_upload_points(h);
+  return assemble_points(h);
 }
 
 int pinn_set_weights(pinn_t* h, const double* w, int64_t n) {
@@ -1445,39 +1436,41 @@ static int forward_ns(pinn_t* h, const double* X, int64_t n, int in_dim, double*
 }
 
 int pinn_predict(pinn_t* h, const double* X, int64_t n, int in_dim, double* out) {
-  if (h && h->pde == PINN_NS_IDE) return forward_ns(h, X, n, in_dim, out, 0);
+  if (h && h->kernel == Kernel::NavierStokes) return forward_ns(h, X, n, in_dim, out, 0);
   return forward_generic(h, X, nullptr, nullptr, n, in_dim, out, 1);
 }
 
 int pinn_derivatives(pinn_t* h, const double* X, int64_t n, double* out) {
-  if (h && h->pde == PINN_NS_IDE) return forward_ns(h, X, n, 3, out, 1);
+  if (h && h->kernel == Kernel::NavierStokes) return forward_ns(h, X, n, 3, out, 1);
   return forward_generic(h, X, nullptr, nullptr, n, h ? h->layers[0] : 2, out, 4);
 }
 
 int64_t pinn_num_residual_points(const pinn_t* h) {
   if (!h) return -1;
-  if (is_disc(h->pde)) return 0;
-  return residual_on_data(h->pde) ? h->n_d : h->n_c;
+  switch (model(h).residual) {
+    case Res::Data: return h->n_d;
+    case Res::Colloc: return h->n_c;
+    case Res::None: break;
+  }
+  return 0;
 }
 
 int pinn_residual(pinn_t* h, double* f_out, int64_t n_rows) {
   if (!h || !f_out) return fail("null argument");
-  if (is_disc(h->pde)) return fail("pinn_residual: not defined for the discrete-time models");
-  if (h->pde == PINN_NS_IDE) {
-    if (n_rows != h->n_d)
-      return fail("pinn_residual: the output buffer holds " + std::to_string(n_rows) + " rows but " + std::to_string(h->n_d) +
-                  " residual points are stored (pinn_num_residual_points)");
-    if (h->n_d == 0) return 0;
-    CUDA_TRY(cudaSetDevice(h->device));
-    return ns_probe(h, h->d_nsX, h->n_d, 2, f_out);
-  }
-  const bool ide = h->pde == PINN_BURGERS_IDE || h->pde == PINN_POLY_IDE;
-  if (is_poly(h->pde) && h->poly.n == 0) return fail("pinn_residual: call pinn_set_residual first (no residual is set)");
-  const int64_t n = ide ? h->n_d : h->n_c;
+  const Res res = model(h).residual;
+  const bool poly = model(h).poly;
+  if (res == Res::None) return fail("pinn_residual: not defined for the discrete-time models");
+  if (poly && h->poly.n == 0) return fail("pinn_residual: call pinn_set_residual first (no residual is set)");
+  const int64_t n = pinn_num_residual_points(h);
   if (n_rows != n)
     return fail("pinn_residual: the output buffer holds " + std::to_string(n_rows) + " rows but " + std::to_string(n) +
                 " residual points are stored (pinn_num_residual_points)");
   if (n == 0) return 0;
+  if (h->kernel == Kernel::NavierStokes) {
+    CUDA_TRY(cudaSetDevice(h->device));
+    return ns_probe(h, h->d_nsX, n, 2, f_out);
+  }
+  const bool ide = res == Res::Data;
   const long long off = ide ? h->dcap - h->n_d : h->dcap;
   std::vector<double> D(n * 4 * h->layers.back());
   const double* rx = (!ide && h->map_x) ? h->map_x : h->d_x + off;
@@ -1493,7 +1486,7 @@ int pinn_residual(pinn_t* h, double* f_out, int64_t n_rows) {
     }
     return 0;
   }
-  if (is_poly(h->pde)) {
+  if (poly) {
     // the kernel head's f, term by term on the host: sum_k c_k kappa_k prod_j v_j^e_kj - s
     double lam[2] = {0.0, 0.0};
     if (ide) CUDA_TRY(cudaMemcpy(lam, h->d_w + h->P_net, 16, cudaMemcpyDeviceToHost));
@@ -1608,24 +1601,28 @@ int pinn_kernel_info(pinn_t* h, char* buf, int buflen) {
   if (!h || !buf || buflen < 1) return fail("bad arguments");
   cudaFuncAttributes fa{};
   int smem = 0, threads = 0;
-  if (h->kernel_kind == 3) {
-    CUDA_TRY(cudaFuncGetAttributes(&fa, pinn::nsid::fused_loss_grad));
-    smem = 0; threads = pinn::nsid::THREADS;
-  } else if (h->kernel_kind == 2) {
-    if (is_poly(h->pde)) CUDA_TRY(cudaFuncGetAttributes(&fa, pinn::generic::fused_loss_grad<true>));
-    else CUDA_TRY(cudaFuncGetAttributes(&fa, pinn::generic::fused_loss_grad<false>));
-    smem = 0; threads = pinn::generic::THREADS;
-  } else if (h->pde == PINN_NLS_INF) {
-    CUDA_TRY(cudaFuncGetAttributes(&fa, pinn::nls::fused_loss_grad));
-    smem = pinn::nls::SMEM_BYTES; threads = pinn::nls::THREADS;
-  } else {
-    if (h->burgers_kernel == 2) {
+  switch (h->kernel) {
+    case Kernel::BurgersV2:
       CUDA_TRY(cudaFuncGetAttributes(&fa, pinn::burgers2::fused_loss_grad));
       smem = pinn::burgers2::SMEM_BYTES; threads = pinn::burgers2::THREADS;
-    } else {
+      break;
+    case Kernel::BurgersV1:
       CUDA_TRY(cudaFuncGetAttributes(&fa, pinn::burgers::fused_loss_grad));
       smem = pinn::burgers::SMEM_BYTES; threads = pinn::burgers::THREADS;
-    }
+      break;
+    case Kernel::Schrodinger:
+      CUDA_TRY(cudaFuncGetAttributes(&fa, pinn::nls::fused_loss_grad));
+      smem = pinn::nls::SMEM_BYTES; threads = pinn::nls::THREADS;
+      break;
+    case Kernel::Generic:
+      if (model(h).poly) CUDA_TRY(cudaFuncGetAttributes(&fa, pinn::generic::fused_loss_grad<true>));
+      else CUDA_TRY(cudaFuncGetAttributes(&fa, pinn::generic::fused_loss_grad<false>));
+      smem = 0; threads = pinn::generic::THREADS;
+      break;
+    case Kernel::NavierStokes:
+      CUDA_TRY(cudaFuncGetAttributes(&fa, pinn::nsid::fused_loss_grad));
+      smem = 0; threads = pinn::nsid::THREADS;
+      break;
   }
   snprintf(buf, buflen, "{\"grid\": %d, \"block\": %d, \"dyn_smem\": %d, \"regs\": %d, \"local_bytes\": %zu, \"sms\": %d}",
            h->n_cta, threads, smem, fa.numRegs, fa.localSizeBytes, h->n_sm);

@@ -119,8 +119,9 @@ def ladder(fam, sms):
 
 
 class CapModel(object):
-    """The capacity rules of pinn_api.cu (ensure_points, pinn_set_data, pinn_set_collocation[_mapped], generic_launch_eval),
-    restated for the continuous-time inference handles, so that a history can be asked what it exercised."""
+    """The capacity rules of pinn_api.cu (ensure_points, upload_points, pinn_set_collocation[_mapped], and Scratch::reserve
+    in generic_launch_eval), restated for the continuous-time inference handles, so that a history can be asked what it
+    exercised."""
 
     def __init__(self, sms):
         self.sms, self.dcap, self.ccap, self.alloc = sms, 0, 0, False

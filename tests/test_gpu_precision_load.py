@@ -48,7 +48,7 @@ def _cdiv(a, b):
 # ------------------------------------------------------------------------------------------------------------------- loads
 # Restatements of the distribution formulas; tests/test_precision_load_cpu.py pins them at 132 SMs.
 def burgers_load(n_total, sms, kernel):
-    """pinn_api.cu:401-404 (grid = min(units, SMs)); v2 splits the tiles of 8 points evenly over the CTAs and each CTA's tiles
+    """pinn_api.cu: burgers_launch_eval (grid = min(units, SMs)); v2 splits the tiles of 8 points evenly over the CTAs and each CTA's tiles
     over its 4 chain warps (burgers_fused_v2.cuh:361-365); v1 stripes rounds of 32 points over the CTAs (burgers_fused.cuh:315)."""
     if kernel == "v2":
         tiles = _cdiv(n_total, 8)
@@ -61,13 +61,13 @@ def burgers_load(n_total, sms, kernel):
 
 
 def nls_load(n_total, sms):
-    """pinn_api.cu:640-642: one CTA per SM, ceil(n / SMs) points rounded up to whole 16-point rounds."""
+    """pinn_api.cu: nls_launch_eval: one CTA per SM, ceil(n / SMs) points rounded up to whole 16-point rounds."""
     pts = _cdiv(_cdiv(n_total, sms), 16) * 16
     return {"points per CTA": pts, "rounds per CTA": pts // 16, "last CTA points": n_total - (_cdiv(n_total, pts) - 1) * pts}
 
 
 def generic_load(n_total, sms):
-    """pinn_api.cu:478-483 with C = 2 x SMs CTAs (pinn_api.cu:856): ceil(n / C) points rounded up to a multiple of 16 from 16
+    """pinn_api.cu: generic_launch_eval with C = 2 x SMs CTAs (pinn_api.cu: pinn_create): ceil(n / C) points rounded up to a multiple of 16 from 16
     on, to an even count below; only CTAs that own points are launched."""
     per = _cdiv(n_total, 2 * sms)
     pts = _cdiv(per, 16) * 16 if per >= 16 else _cdiv(per, 2) * 2
@@ -77,14 +77,14 @@ def generic_load(n_total, sms):
 
 
 def ns_load(n_total, sms):
-    """pinn_api.cu:550-551: one CTA per SM, ceil(n / SMs) points each, in M tiles of 16 points."""
+    """pinn_api.cu: ns_launch_eval: one CTA per SM, ceil(n / SMs) points each, in M tiles of 16 points."""
     pts = _cdiv(n_total, sms)
     grid = _cdiv(n_total, pts)
     return {"points per CTA": pts, "M tiles per CTA": _cdiv(pts, 16), "grid": grid, "last CTA points": n_total - (grid - 1) * pts}
 
 
 def ns_probe_chunks(n, maxw):
-    """pinn_api.cu:594-601: chunks of (32 Mi) / (2 x 13 x maxw) points."""
+    """pinn_api.cu: ns_probe: chunks of (32 Mi) / (2 x 13 x maxw) points."""
     chunk = min((32 << 20) // (2 * 13 * maxw), n)
     return {"chunk": chunk, "chunks": _cdiv(n, chunk), "last chunk": n - (_cdiv(n, chunk) - 1) * chunk}
 

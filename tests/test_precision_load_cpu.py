@@ -148,7 +148,7 @@ SMS = 132
 
 
 def test_burgers_loads():
-    # pinn_api.cu:401-404, burgers_fused_v2.cuh:361-365, burgers_fused.cuh:315
+    # pinn_api.cu: burgers_launch_eval; burgers_fused_v2.cuh:361-365, burgers_fused.cuh:315
     assert burgers_load(100100, SMS, "v2") == {"grid": 132, "tiles per CTA": 95, "rounds per chain warp": 24}
     assert burgers_load(100100, SMS, "v1") == {"grid": 132, "rounds per CTA": 24}
     assert burgers_load(2000100, SMS, "v2") == {"grid": 132, "tiles per CTA": 1895, "rounds per chain warp": 474}
@@ -157,14 +157,14 @@ def test_burgers_loads():
 
 
 def test_schrodinger_loads():
-    # pinn_api.cu:640-642: the upstream 20 000 + 50 + 2 x 50 points take 10 rounds per CTA
+    # pinn_api.cu: nls_launch_eval: the upstream 20 000 + 50 + 2 x 50 points take 10 rounds per CTA
     assert nls_load(20150, SMS) == {"points per CTA": 160, "rounds per CTA": 10, "last CTA points": 150}
     assert nls_load(106150, SMS)["rounds per CTA"] == 51
     assert nls_load(1950, SMS)["rounds per CTA"] == 1
 
 
 def test_generic_loads():
-    # pinn_api.cu:478-483, C = 264 CTAs
+    # pinn_api.cu: generic_launch_eval, C = 264 CTAs
     assert generic_load(16 * 264 - 1, SMS) == {"points per CTA": 16, "8-point groups per CTA": 2, "grid": 264,
                                                "last CTA points": 15}
     assert generic_load(16 * 264 + 1, SMS) == {"points per CTA": 32, "8-point groups per CTA": 4, "grid": 133,
@@ -175,7 +175,7 @@ def test_generic_loads():
 
 
 def test_navier_stokes_loads():
-    # pinn_api.cu:550-551 and, for the probe, 594-601
+    # pinn_api.cu: ns_launch_eval and, for the probe, ns_probe
     assert ns_load(5000, SMS) == {"points per CTA": 38, "M tiles per CTA": 3, "grid": 132, "last CTA points": 22}
     assert ns_load(50000, SMS) == {"points per CTA": 379, "M tiles per CTA": 24, "grid": 132, "last CTA points": 351}
     assert ns_probe_chunks(16000, 256) == {"chunk": 5041, "chunks": 4, "last chunk": 877}
