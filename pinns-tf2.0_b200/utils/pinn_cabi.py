@@ -299,6 +299,13 @@ class Pinn(object):
     def derivatives(self, X):
         """(u, u_x, u_t, u_xx), each (n, out_dim).  NS_IDE: one (n, 13, 2) array, the streams of NS_STREAMS, each (psi, p)."""
         X = _arr(X)
+        if X.ndim == 1:
+            X = X[:, None]
+        if X.shape[1] == 1 and self.layers[0] == 2:
+            X = np.concatenate([X, X], axis=1)      # quirk Q1, as predict: an (n, 1) input is (x, t := x)
+        if X.shape[1] != self.layers[0]:
+            raise PinnError(f"derivatives: X has {X.shape[1]} columns, the net takes {self.layers[0]}")
+        X = np.ascontiguousarray(X)
         if self.pde == NS_IDE:
             out = np.empty((X.shape[0], len(NS_STREAMS), 2))
             self._ck(self.lib.pinn_derivatives(self.h, _p(X), X.shape[0], _p(out)))

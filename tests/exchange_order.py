@@ -15,7 +15,8 @@ import numpy as np
 
 TESTS = os.path.dirname(os.path.abspath(__file__))
 PKG = os.path.join(os.path.dirname(TESTS), "pinns-tf2.0_b200")
-CSRC = os.path.join(PKG, "csrc")
+# PINN_CSRC: the kernel sources of another build of the library (PINN_LIB), e.g. a mutant of tests/kernel_mutants.py
+CSRC = os.environ.get("PINN_CSRC") or os.path.join(PKG, "csrc")
 SOURCE = os.path.join(TESTS, "exchange_harness.cu")
 P2P_MAX = 8
 RING = 16                        # loss ring entries of the harness

@@ -98,9 +98,15 @@ try:
 except UnboundLocalError:
     print("%-34s reference raises UnboundLocalError (t unassigned); port reports 'no progress'" % "no progress at iteration 1")
 
+sys.path.insert(0, ROOT + "/tests")
+# Every stop test and the curvature test with its operands exactly on the threshold (tests/test_gpu_lbfgs_foreign.py holds the
+# device L-BFGS to the port on the same set): which side of each comparison counts is the reference's.
+from test_gpu_lbfgs_foreign import BOUNDARY_CASES  # noqa: E402
+for name, fn, x0, reason, kw in BOUNDARY_CASES:
+    compare(name, fn, x0, reason, **kw)
+
 # Objectives whose f, g or both turn NaN or +-Inf at evaluation 0, 1 or 4 (tests/test_gpu_nonfinite.py holds the device L-BFGS
 # to the port on the same set): stop reason, counts, logged iterations and every point asked for, NaN-aware.
-sys.path.insert(0, ROOT + "/tests")
 from test_gpu_nonfinite import LBFGS_KW, LBFGS_OBJECTIVES, LBFGS_X0, nonfinite_objective  # noqa: E402
 for name, k, at, wh in LBFGS_OBJECTIVES:
     kw = dict(maxIter=LBFGS_KW["max_iter"], learningRate=LBFGS_KW["lr"], nCorrection=LBFGS_KW["n_corr"], tolFun=LBFGS_KW["tol_fun"])

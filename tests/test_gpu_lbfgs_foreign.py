@@ -72,6 +72,33 @@ CASES = [
 ]
 
 
+def two_valued(first, later):
+    """(f, g) = first at the start point (x[0] == 0) and later everywhere else.  The values are dyadic with one nonzero gradient
+    entry, so |g|_1, |d t|_1, g.d, y.s and f - f_old are exact in any summation order and land exactly on a threshold."""
+    return lambda x: (first[0], np.array(first[1])) if x[0] == 0.0 else (later[0], np.array(later[1]))
+
+
+TINY = 2.0 ** -20     # g = (-TINY, 0) at the start: the first step is s = (TINY, 0), so y.s = y_0 TINY exactly
+# Each stop test and the curvature test with its operands exactly on the threshold (the reference's custom_lbfgs.py decides the
+# side, tests/test_reference_pin.py).  The expected reason is the product's; the other side of the comparison ends elsewhere.
+BOUNDARY_CASES = [
+    ("g1_eq_tolfun_at_start", two_valued((1.0, [0.25, 0.0]), (0.5, [0.25, 0.0])), [0.0, 0.0], "initial optimality",
+     dict(maxIter=5, tolFun=0.25)),
+    ("g1_eq_tolfun_after_a_step", two_valued((1.0, [0.5, 0.0]), (0.5, [0.25, 0.0])), [0.0, 0.0], "optimality",
+     dict(maxIter=5, tolFun=0.25)),
+    ("step_eq_tolx", two_valued((4.0, [2.0, 0.0]), (0.0, [2.0, 0.0])), [0.0, 0.0], "step below tolX", dict(maxIter=5, tolX=1.0)),
+    ("f_change_eq_tolx", two_valued((1.0, [1.0, 0.0]), (0.75, [1.0, 0.0])), [0.0, 0.0], "max iterations",
+     dict(maxIter=2, tolX=0.25)),
+    ("gtd_eq_minus_tolx", two_valued((1.0, [0.5, 0.0]), (0.0, [0.5, 0.0])), [0.0, 0.0], "max iterations",
+     dict(maxIter=2, tolX=0.25)),
+    ("ys_eq_1e-10_rejected", two_valued((1.0, [-TINY, 0.0]), (0.5, [1e-10 / TINY - TINY, 0.0])), [0.0, 0.0],
+     "f change below tolX", dict(maxIter=4, tolFun=1e-30)),
+    ("ys_2^-31_accepted", two_valued((1.0, [-TINY, 0.0]), (0.5, [2.0 ** -11 - TINY, 0.0])), [0.0, 0.0],
+     "f change below tolX", dict(maxIter=4, tolFun=1e-30)),
+]
+CASES += BOUNDARY_CASES
+
+
 @pytest.mark.parametrize("name,fn,x0,reason,kw", CASES, ids=[c[0] for c in CASES])
 def test_foreign_closure_takes_every_exit_like_the_reference(name, fn, x0, reason, kw):
     compare(fn, x0, reason, **kw)

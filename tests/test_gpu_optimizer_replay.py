@@ -32,6 +32,7 @@ import pytest
 
 from conftest import ROOT, load_golden
 from oracle import reference_port as rp
+from test_gpu_lbfgs_foreign import BOUNDARY_CASES
 
 pytestmark = pytest.mark.gpu
 
@@ -295,8 +296,10 @@ def lbfgs_replay(run, x0, mode, max_iter, lr=1.0, n_corr=100, tol_fun=1e-5, tol_
             # other side of the threshold: within |y| |s_dev - s_ld| (the step it took differs from the replay's) plus the
             # rounding of the dot product.  The replay cannot know which branch the kernel took; it stops there.
             ys, ys_abs = ld.curv[k - 1]
+            # One nonzero product and a step equal to the replay's: the kernel's y.s is the replay's, even on the threshold.
             y = np.asarray(run["gs"][k], dtype=LD) - np.asarray(run["gs"][k - 1], dtype=LD)
-            if abs(float(ys) - 1e-10) <= nrm(y) * s_prev + 1e-12 * float(ys_abs):
+            exact = s_prev == 0.0 and np.count_nonzero(y * (LD(ld.t[k - 1]) * ld.d[k - 1])) <= 1
+            if not exact and abs(float(ys) - 1e-10) <= nrm(y) * s_prev + 1e-12 * float(ys_abs):
                 undetermined = k + 1
                 break
         s_ld = LD(ld.t[k]) * ld.d[k]
@@ -367,6 +370,10 @@ LBFGS_CASES = [
     ("first_step_g1_below_1", quad3, 0.999 * X3, 6, dict(lr=0.5, tol_fun=1e-30)),
     ("first_step_g1_above_1", quad3, 1.001 * X3, 6, dict(lr=0.5, tol_fun=1e-30)),
 ]
+# every stop test and the curvature test exactly on its threshold (test_gpu_lbfgs_foreign.BOUNDARY_CASES), in both kernels
+_KW = {"maxIter": "max_iter", "learningRate": "lr", "nCorrection": "n_corr", "tolFun": "tol_fun", "tolX": "tol_x"}
+LBFGS_CASES += [(name, fn, np.array(x0), kw["maxIter"], {_KW[k]: v for k, v in kw.items() if k != "maxIter"})
+                for name, fn, x0, _, kw in BOUNDARY_CASES]
 GRAM_ONLY = ("gram_n40000", "gram_n100000")
 # the golden Burgers PINN (the problem of profiles/run_lbfgs_stability.py) after ADAM_EPOCHS Adam steps at lr 0.03, then
 # BURGERS_ITERS fixed steps of 0.8 with a 50-pair history

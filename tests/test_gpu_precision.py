@@ -422,6 +422,31 @@ def test_probes_per_stream(cabi, case):
     print("[precision] %-40s worst error/bound %.3g" % ("probes/" + name, max(worst, r)))
 
 
+@pytest.mark.parametrize("model", ["burgers", "nls"])
+def test_probes_on_one_column_input(cabi, model):
+    """Quirk Q1: an (n, 1) input to a 2-D net is broadcast to (x, t := x) by the reference's Lambda.  predict takes it as it is
+    (the probe kernel reads t := x), derivatives broadcasts it on the host; both equal the oracle on (x, x).  x spans the box's
+    x range, so t := x lies outside the t range on purpose."""
+    layers, pde, (lb, ub) = (BURGERS, cabi.BURGERS_INF, DOMAINS["shifted"]) if model == "burgers" else (NLS, cabi.NLS_INF, NLS_OTHER)
+    lb, ub = np.array(lb), np.array(ub)
+    x = np.random.default_rng(450).uniform(lb[0], ub[0], (200, 1))
+    w = load_golden("nls_inf" if model == "nls" else "burgers_inf")["w"]
+    p = cabi.Pinn(pde, layers, lb, ub)
+    p.set_weights(w)
+    pred, got = p.predict(x), p.derivatives(x)
+    with pytest.raises(cabi.PinnError, match="columns"):
+        p.derivatives(np.zeros((4, 3)))
+    p.close()
+    XX = np.concatenate([x, x], 1)
+    ref, _ = ty.forward(w, layers, lb, ub, XX, dtype=LD)
+    ref64, _ = ty.forward(w, layers, lb, ub, XX)
+    bound = lambda s, o, tol: tol * _norm(ref[s][:, o]) + FP64_FACTOR * _norm(ref64[s][:, o] - ref[s][:, o])
+    for o in range(layers[-1]):
+        assert _ratio(_norm(pred[:, o] - ref[0][:, o]), bound(0, o, PROBE_TOL[0])) <= 1.0, (model, "predict", o)
+        for s, tol in enumerate(PROBE_TOL):
+            assert _ratio(_norm(got[s][:, o] - ref[s][:, o]), bound(s, o, tol)) <= 1.0, (model, "derivatives", s, o)
+
+
 # ------------------------------------------------------------------------------- L-BFGS kernel instantiation switch points
 # pinn_api.cu picks lbfgs_iterate<12,256> for P <= 3072, <8,1024> for P <= 8192 and <32,1024> above
 @pytest.mark.parametrize("layers", [[2, 13, 43, 54, 1], [2, 52, 54, 1], [2, 31, 104, 45, 1], [2, 32, 104, 44, 1]],

@@ -300,7 +300,8 @@ def test_gpu_tests_reference_run_keys_exist():
 @pytest.mark.skipif(not os.path.isdir(REF), reason="needs an upstream PINNs-TF2.0 checkout named by PINNS_TF2_REFERENCE")
 def test_lbfgs_control_flow_equals_the_reference():
     """Every exit of the reference's lbfgs() (maxIter, maxEval, optimality at the start / later, no progress, step below tolX,
-    f change below tolX) plus rejected curvature pairs and history overflow: evaluation points, f history, returned x, logged
+    f change below tolX) plus rejected curvature pairs and history overflow, and every stop and curvature test with its operands
+    exactly on the threshold (test_gpu_lbfgs_foreign.BOUNDARY_CASES): evaluation points, f history, returned x, logged
     iterations, evaluation and iteration counts of oracle.reference_port.lbfgs_fixed_step equal the reference's on synthetic
     objectives.  One known difference: 'no progress' at the very first iteration is an UnboundLocalError in the reference."""
     r = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "lbfgs_compare_worker.py"), ROOT],
