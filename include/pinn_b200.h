@@ -130,6 +130,20 @@ int pinn_set_collocation(pinn_t* h, const double* x, const double* t, int64_t n,
  * The buffers must stay valid and unchanged until the next synchronising call.  Burgers inference kernel only. */
 int pinn_set_collocation_mapped(pinn_t* h, const double* x_pinned, const double* t_pinned, int64_t n, int64_t n_global);
 
+/* BURGERS_INF, NLS_INF, POLY_INF: replace this rank's collocation set by rows [first, first + n) of Latin-hypercube draw `draw`
+ * of `seed` over [lb, ub] of pinn_create, with N = n_global strata per dimension (DESIGN §4.6).  Enqueue only: no host buffer,
+ * no synchronisation (except when the collocation region has to grow, as for pinn_set_collocation).  n_global is also the MSE_f
+ * denominator, as in pinn_set_collocation; 1 <= n_global <= 2^53 and 0 <= first <= first + n <= n_global.  Replaces a mapped
+ * batch.  POLY_INF: the source resets to zero, like every new set of residual points.  The drawn set is a current input of the
+ * handle, defined by (seed, draw, first, n, n_global, lb, ub): the handle equals a fresh one fed the same points through
+ * pinn_set_collocation.  The row rule: one Philox4x32-10 block of (row, draw) under the seed gives two 53-bit uniforms, two
+ * keyed Feistel permutations of [0, n_global) give the strata, and x_d = lb_d + (ub_d - lb_d) * ((stratum + u) / n_global). */
+int pinn_draw_collocation(pinn_t* h, uint64_t seed, uint64_t draw, int64_t first, int64_t n, int64_t n_global);
+/* The stored collocation set, however it got there (upload, mapped batch, draw): x, t hold n doubles each; n must equal
+ * pinn_num_residual_points(h).  Synchronises.  A POLY_INF caller with a source reads a drawn set back here, evaluates s(x, t)
+ * and calls pinn_set_source. */
+int pinn_get_collocation(pinn_t* h, double* x, double* t, int64_t n);
+
 /* Data term: X_u,u of fit(X_u,u) (utils/neuralnetwork.py:138-146).  X is (n,in_dim) row-major; in_dim==1
  * reproduces the Lambda's broadcast of a (N,1) input to (x, t:=x) (quirk Q1, inf_cont_schrodinger.py:164).
  * u is (n,out_dim).  For BURGERS_IDE these are also the residual points (ide_cont_burgers.py:88-91,116-118).

@@ -18,6 +18,7 @@
 #include "optim_kernels.cuh"
 #include "generic_fused.cuh"
 #include "navier_stokes_fused.cuh"
+#include "lhs_draw.cuh"
 
 namespace {
 
@@ -1108,6 +1109,53 @@ int pinn_set_collocation(pinn_t* h, const double* x, const double* t, int64_t n,
   h->n_c = n; h->n_c_global = n_global;
   h->map_x = h->map_t = nullptr;
   h->h_src.clear();                               // POLY_INF: new residual points, the source is 0 until set again
+  return 0;
+}
+
+int pinn_draw_collocation(pinn_t* h, uint64_t seed, uint64_t draw, int64_t first, int64_t n, int64_t n_global) {
+  if (!h) return fail("null handle");
+  if (model(h).residual == Res::Data)
+    return fail("pinn_draw_collocation: identification uses the data points as residual points");
+  if (model(h).residual == Res::None)
+    return fail("pinn_draw_collocation: the discrete-time models have no collocation set (snapshot / boundary points only)");
+  if (n_global < 1 || n_global > (1LL << 53)) return fail("pinn_draw_collocation: n_global must be in 1..2^53");
+  if (first < 0 || n < 0 || first > n_global || n > n_global - first)
+    return fail("pinn_draw_collocation: the rows [first, first + n) must lie in [0, n_global)");
+  CUDA_TRY(cudaSetDevice(h->device));
+  if (ensure_points(h, h->n_aux, n)) return -1;
+  if (n) {
+    pinn::lhs::Args a{};
+    a.x = h->d_x + h->dcap; a.t = h->d_t + h->dcap;
+    a.seed = seed; a.draw = draw; a.first = (uint64_t)first; a.n = (uint64_t)n; a.n_global = (uint64_t)n_global;
+    a.lb0 = h->lb[0]; a.lb1 = h->lb[1]; a.dx0 = h->ub[0] - h->lb[0]; a.dx1 = h->ub[1] - h->lb[1];
+    a.m = pinn::lhs::half_bits((uint64_t)n_global);
+    const long long blocks = (n + pinn::lhs::THREADS - 1) / pinn::lhs::THREADS;
+    const int grid = (int)(blocks < 8LL * h->n_sm ? blocks : 8LL * h->n_sm);     // one wave of 256-thread blocks, grid-stride beyond
+    pinn::lhs::draw_kernel<<<grid, pinn::lhs::THREADS, 0, h->stream>>>(a);
+    CUDA_TRY(cudaGetLastError());
+    h->launches++;
+  }
+  h->n_c = n; h->n_c_global = n_global;
+  h->map_x = h->map_t = nullptr;
+  h->h_src.clear();                               // POLY_INF: new residual points, the source is 0 until set again
+  return 0;
+}
+
+int pinn_get_collocation(pinn_t* h, double* x, double* t, int64_t n) {
+  if (!h) return fail("null handle");
+  if (model(h).residual != Res::Colloc) return fail("pinn_get_collocation: this model has no collocation set");
+  if (n != h->n_c)
+    return fail("pinn_get_collocation: the output buffers hold " + std::to_string(n) + " rows but " + std::to_string(h->n_c) +
+                " collocation points are stored (pinn_num_residual_points)");
+  if (n == 0) return 0;
+  if (!x || !t) return fail("pinn_get_collocation: null argument");
+  CUDA_TRY(cudaSetDevice(h->device));
+  // a mapped batch is read through its device alias: the copy is ordered after the launches that still read it
+  const double* sx = h->map_x ? h->map_x : h->d_x + h->dcap;
+  const double* st = h->map_t ? h->map_t : h->d_t + h->dcap;
+  CUDA_TRY(cudaMemcpyAsync(x, sx, (size_t)n * 8, cudaMemcpyDefault, h->stream));
+  CUDA_TRY(cudaMemcpyAsync(t, st, (size_t)n * 8, cudaMemcpyDefault, h->stream));
+  CUDA_TRY(cudaStreamSynchronize(h->stream));
   return 0;
 }
 

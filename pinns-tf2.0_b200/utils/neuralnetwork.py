@@ -139,6 +139,11 @@ class NeuralNetwork(object):
                 self.sizes_w.append(int(width * layers[1]))
                 self.sizes_b.append(int(width if i != 0 else layers[1]))
         self.logger = logger
+        # optional per-step resampling of the collocation set on the device (not in the reference): before Adam epoch e > 0
+        # with e % resample_every == 0 the set is replaced by Latin-hypercube draw e // resample_every of resample_seed
+        self.resample_every = _hp_int(hp, "resample_every", 0, 0)
+        self.resample_seed = _hp_int(hp, "resample_seed", 0, 0, 1 << 64)
+        self._tf_epoch = 0
         self._h = None
         self._w0 = _glorot_normal(self.layers, np.random.default_rng(self.weight_seed))
         self._bound = None
@@ -201,6 +206,8 @@ class NeuralNetwork(object):
     def _native(self):
         if self._h is None:
             pde = self._pde_id()
+            if self.resample_every and pde not in _COLLOCATION:
+                raise pinn_cabi.PinnError('hp["resample_every"]: %s has no collocation set to resample' % type(self).__name__)
             h = pinn_cabi.Pinn(pde, self.layers, self.lb, self.ub, device=getattr(self, "device", 0),
                                rank=getattr(self, "rank", 0), world=getattr(self, "world", 1),
                                nccl_uid=getattr(self, "nccl_uid", None))
@@ -338,18 +345,35 @@ class NeuralNetwork(object):
         return loss_and_flat_grad
 
     def tf_optimization(self, X_u, u):
+        """Adam epochs.  With hp["resample_every"] = k the collocation set is redrawn on the device before every epoch e > 0 with
+        e % k == 0 (tf_optimization_step); epochs [0, k) train on the script's own X_f, and the L-BFGS phase that follows runs on
+        the last drawn set."""
         self.logger.log_train_opt("Adam")
+        self._tf_epoch = 0
         for epoch in range(self.tf_epochs):
             loss_value = self.tf_optimization_step(X_u, u)
             self.logger.log_train_epoch(epoch, loss_value)
 
     def tf_optimization_step(self, X_u, u):
-        """One fused loss/grad evaluation + on-device Adam update, enqueued without a host sync."""
+        """One fused loss/grad evaluation + on-device Adam update, enqueued without a host sync.  With hp["resample_every"] = k,
+        epoch e > 0 with e % k == 0 first replaces the collocation set by Latin-hypercube draw e // k of hp["resample_seed"] over
+        the script's N_f points (n_f_global when sharded), this rank's rows of it (pinn_draw_collocation)."""
         self._bind(X_u, u)
         n = self._native()
+        e, k = self._tf_epoch, self.resample_every
+        if k and e > 0 and e % k == 0:
+            self._resample(n, e // k)
+        self._tf_epoch = e + 1
         n.adam_step(self.tf_lr, self.tf_b1, self.tf_b2, self.tf_eps, sync=False)
         self._adam_serial = getattr(self, "_adam_serial", 0) + 1
         return LazyLoss(n, self)
+
+    def _resample(self, n, draw):
+        n_global = getattr(self, "n_f_global", None) or int(np.asarray(self.x_f).shape[0])
+        n.draw_collocation(self.resample_seed, draw, n_global, rank=getattr(self, "rank", 0), world=getattr(self, "world", 1))
+        if n.pde == pinn_cabi.POLY_INF and callable(getattr(self, "source", None)):
+            x, t = n.get_collocation()                       # the one host round trip a source needs
+            self._upload_source(np.stack([x, t], 1), n)
 
     def nt_optimization(self, X_u, u):
         self.logger.log_train_opt("LBFGS")
@@ -396,6 +420,17 @@ _TWO_SNAPSHOT = (pinn_cabi.BURGERS_IDE_DISC, pinn_cabi.KDV_IDE_DISC)
 _LAMBDAS = (pinn_cabi.BURGERS_IDE, pinn_cabi.NS_IDE, pinn_cabi.POLY_IDE) + _TWO_SNAPSHOT
 # user-defined polynomial residuals (pde = "poly")
 _POLY = (pinn_cabi.POLY_INF, pinn_cabi.POLY_IDE)
+# models with a collocation set (pinn_set_collocation, pinn_draw_collocation)
+_COLLOCATION = (pinn_cabi.BURGERS_INF, pinn_cabi.NLS_INF, pinn_cabi.POLY_INF)
+
+
+def _hp_int(hp, key, default, lo, hi=None):
+    """An optional integer hyper-parameter in [lo, hi)."""
+    v = hp.get(key, default) if hasattr(hp, "get") else default
+    v = default if v is None else v
+    if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)) or v < lo or (hi is not None and v >= hi):
+        raise pinn_cabi.PinnError('hp["%s"] = %r: expected an integer >= %d%s' % (key, v, lo, "" if hi is None else " below %d" % hi))
+    return int(v)
 
 
 def _scalar(v):

@@ -9,6 +9,8 @@ import os
 
 import numpy as np
 
+from sharding import shard_rows
+
 _HERE = os.path.dirname(os.path.realpath(__file__))
 # PINN_LIB: load another build of the same library (kernel experiments: profiles/kernel_variants.py)
 LIB_PATH = os.environ.get("PINN_LIB") or os.path.join(_HERE, "..", "lib", "libpinn_b200.so")
@@ -43,6 +45,8 @@ SIGNATURES = {
     "pinn_set_irk": (C.c_int, [C.c_void_p, _dp, C.c_int]),
     "pinn_set_collocation": (C.c_int, [C.c_void_p, _dp, _dp, C.c_int64, C.c_int64]),
     "pinn_set_collocation_mapped": (C.c_int, [C.c_void_p, _dp, _dp, C.c_int64, C.c_int64]),
+    "pinn_draw_collocation": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, C.c_int64, C.c_int64, C.c_int64]),
+    "pinn_get_collocation": (C.c_int, [C.c_void_p, _dp, _dp, C.c_int64]),
     "pinn_set_data": (C.c_int, [C.c_void_p, _dp, C.c_int64, C.c_int, _dp, C.c_int, C.c_double]),
     "pinn_set_snapshot": (C.c_int, [C.c_void_p, C.c_int, _dp, C.c_int64, _dp]),
     "pinn_set_boundary": (C.c_int, [C.c_void_p, _dp, C.c_int64]),
@@ -200,6 +204,22 @@ class Pinn(object):
     def set_collocation_mapped(self, x_ptr, t_ptr, n, n_global=None):
         """Zero-copy: the fused kernel reads the (pinned) host buffers directly; keep them alive and unchanged."""
         self._ck(self.lib.pinn_set_collocation_mapped(self.h, x_ptr, t_ptr, int(n), int(n_global or n)))
+
+    def draw_collocation(self, seed, draw, n_global, rank=0, world=1):
+        """Replace the collocation set by this rank's rows (sharding.shard_rows) of Latin-hypercube draw `draw` of `seed`, with
+        n_global strata per dimension over [lb, ub] (pinn_draw_collocation).  Enqueued on the device; nothing is synchronised."""
+        for name, v in (("seed", seed), ("draw", draw)):
+            if not 0 <= int(v) < 1 << 64:
+                raise PinnError(f"draw_collocation: {name} = {int(v)} is not an unsigned 64-bit integer")
+        first, hi = shard_rows(int(n_global), int(rank), int(world))
+        self._ck(self.lib.pinn_draw_collocation(self.h, int(seed), int(draw), first, hi - first, int(n_global)))
+
+    def get_collocation(self):
+        """(x, t) of the stored collocation set, however it got there (upload, mapped batch, draw)."""
+        n = int(self.lib.pinn_num_residual_points(self.h))
+        x, t = np.empty(n), np.empty(n)
+        self._ck(self.lib.pinn_get_collocation(self.h, _p(x), _p(t), n))
+        return x, t
 
     def set_data(self, X, u, weight=1.0):
         X, u = _arr(X), _arr(u)
