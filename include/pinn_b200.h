@@ -139,6 +139,28 @@ int pinn_set_collocation_mapped(pinn_t* h, const double* x_pinned, const double*
  * pinn_set_collocation.  The row rule: one Philox4x32-10 block of (row, draw) under the seed gives two 53-bit uniforms, two
  * keyed Feistel permutations of [0, n_global) give the strata, and x_d = lb_d + (ub_d - lb_d) * ((stratum + u) / n_global). */
 int pinn_draw_collocation(pinn_t* h, uint64_t seed, uint64_t draw, int64_t first, int64_t n, int64_t n_global);
+/* BURGERS_INF, NLS_INF, one GPU: residual-based adaptive resampling (RAD, Wu et al., CMAME 403, 2023; DESIGN §4.7).  Replaces
+ * the collocation set by n points drawn, with replacement, from a pool with probability proportional to a quantised
+ * eps(x)^k / E[eps^k] + c, where eps is the PDE residual at the handle's current weights.  Enqueue only, like
+ * pinn_draw_collocation: no host buffer, no synchronisation (except when the collocation region or the pool scratch has to grow).
+ * n is also the MSE_f denominator.  Replaces a mapped batch.  The handle then equals a fresh one fed the same points through
+ * pinn_set_collocation.  The draw, step by step (every integer step is exact, so it does not depend on a reduction order):
+ *   1. pool: rows [0, n_pool) of Latin-hypercube draw `draw` of `seed` with n_pool strata, i.e. what
+ *      pinn_draw_collocation(h, seed, draw, 0, n_pool, n_pool) stores;
+ *   2. f_i at pool point i, from the weights after every step already enqueued: bit for bit the value pinn_residual returns;
+ *   3. r_i = |f_i| (BURGERS_INF) or sqrt(f_u^2 + f_v^2) (NLS_INF), each operation rounded; a_i = r_i^k as left-to-right rounded
+ *      products (k = 0: a_i = 1);
+ *   4. amax = the largest finite a_i (0 if none); A_i = 2^24 if a_i is not finite, else floor((a_i / amax) * 2^24) as a uint64
+ *      (0 when amax = 0); S = sum A_i; C' = floor(c * (double)S / n_pool) (one rounded fp64 multiply, one rounded divide);
+ *      Q_i = A_i + C', T = sum Q_i, and every Q_i = 1 if T = 0;
+ *   5. row j: one Philox4x32-10 block (w0, w1, w2, w3) with counter (lo j, hi j, lo draw, hi draw) and key
+ *      (lo seed ^ 0xBF58476D, hi seed ^ 0x1CE4E5B9); target = mulhi64(w0 << 32 | w1, T), in [0, T); row j is pool point i for
+ *      the least i whose inclusive prefix Q_0 + ... + Q_i exceeds target.
+ * Points with Q_i = 0 are never drawn; a non-finite residual takes the largest weight.  Up to the 2^-24 quantisation Q_i / T is
+ * RAD's (a_i / mean a + c) / (n_pool (1 + c)).  Unlike Wu et al. the draw is with replacement: a point may appear more than once.
+ * Refused (the handle is left unchanged) for the identification, discrete-time and Navier-Stokes models, for POLY_INF (its
+ * source lives on the host), for world > 1, and unless 0 <= k <= 4, c is finite in [0, 1024], 1 <= n_pool <= 2^29 and n >= 0. */
+int pinn_draw_collocation_rad(pinn_t* h, uint64_t seed, uint64_t draw, int64_t n_pool, int64_t n, int k, double c);
 /* The stored collocation set, however it got there (upload, mapped batch, draw): x, t hold n doubles each; n must equal
  * pinn_num_residual_points(h).  Synchronises.  A POLY_INF caller with a source reads a drawn set back here, evaluates s(x, t)
  * and calls pinn_set_source. */

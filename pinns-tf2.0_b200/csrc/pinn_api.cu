@@ -19,6 +19,7 @@
 #include "generic_fused.cuh"
 #include "navier_stokes_fused.cuh"
 #include "lhs_draw.cuh"
+#include "rad_sample.cuh"
 
 namespace {
 
@@ -291,6 +292,8 @@ struct pinn_handle {
   long long pscr_cap = 0;
   double* d_nsX = nullptr;                  // NS: training points [n][3] = (x, y, t); targets [n][2] in d_u
   long long nsx_cap = 0;
+  double* d_rad = nullptr;                  // pinn_draw_collocation_rad: pool x, t, r^k, segment prefixes, block maxima and sums
+  long long rad_cap = 0;
 
   // POLY_INF / POLY_IDE: the residual's term table (n == 0: not set yet) and the source at the residual points (empty: 0)
   pinn::generic::PolySpec poly{};
@@ -994,7 +997,7 @@ int pinn_destroy(pinn_t* h) {
   if (h->d_xseq) cudaFree(h->d_xseq);
   if (h->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(h->comm);
   double* bufs[] = {h->d_w, h->d_R, h->d_partials, h->d_m, h->d_v, h->d_loss_ring, h->d_x, h->d_t, h->d_u, h->d_irk,
-                    h->d_px, h->d_pout, h->d_pscr, h->d_nsX, h->d_src};
+                    h->d_px, h->d_pout, h->d_pscr, h->d_nsX, h->d_src, h->d_rad};
   for (double* b : bufs) if (b) cudaFree(b);
   if (h->d_step) cudaFree(h->d_step);
   h->scratch.release();
@@ -1138,6 +1141,69 @@ int pinn_draw_collocation(pinn_t* h, uint64_t seed, uint64_t draw, int64_t first
   h->n_c = n; h->n_c_global = n_global;
   h->map_x = h->map_t = nullptr;
   h->h_src.clear();                               // POLY_INF: new residual points, the source is 0 until set again
+  return 0;
+}
+
+static int launch_forward_generic(pinn_t* h, const double* dx, const double* dt, int64_t n, int in_dim, int ns);
+
+int pinn_draw_collocation_rad(pinn_t* h, uint64_t seed, uint64_t draw, int64_t n_pool, int64_t n, int k, double c) {
+  if (!h) return fail("null handle");
+  const Model& m = model(h);
+  if (m.residual == Res::Data)
+    return fail("pinn_draw_collocation_rad: identification uses the data points as residual points");
+  if (m.residual == Res::None)
+    return fail("pinn_draw_collocation_rad: the discrete-time models have no collocation set (snapshot / boundary points only)");
+  if (m.poly)
+    return fail("pinn_draw_collocation_rad: POLY_INF's source s(x, t) lives on the host, so its residual cannot be formed on a "
+                "pool drawn on the device");
+  if (h->world > 1)
+    return fail("pinn_draw_collocation_rad: runs on one GPU (world must be 1): the weights are normalised over the whole pool");
+  if (k < 0 || k > 4) return fail("pinn_draw_collocation_rad: k must be in 0..4");
+  if (!(c >= 0.0 && c <= pinn::rad::MAX_C)) return fail("pinn_draw_collocation_rad: c must be finite and in [0, 1024]");
+  if (n_pool < 1 || n_pool > pinn::rad::MAX_POOL) return fail("pinn_draw_collocation_rad: n_pool must be in 1..2^29");
+  if (n < 0) return fail("pinn_draw_collocation_rad: n must be >= 0");
+  CUDA_TRY(cudaSetDevice(h->device));
+  if (n) {
+    using namespace pinn;
+    const long long blocks = (n_pool + rad::THREADS - 1) / rad::THREADS;
+    const int grid = (int)(blocks < rad::MAX_BLOCKS ? blocks : rad::MAX_BLOCKS);
+    if (ensure(&h->d_rad, &h->rad_cap, 4 * n_pool + 2 * rad::MAX_BLOCKS)) return -1;
+    if (ensure_points(h, h->n_aux, n)) return -1;
+    double* px = h->d_rad;
+    double* pt = px + n_pool;
+    // the pool: what pinn_draw_collocation(seed, draw, 0, n_pool, n_pool) stores
+    lhs::Args l{};
+    l.x = px; l.t = pt;
+    l.seed = seed; l.draw = draw; l.first = 0; l.n = (uint64_t)n_pool; l.n_global = (uint64_t)n_pool;
+    l.lb0 = h->lb[0]; l.lb1 = h->lb[1]; l.dx0 = h->ub[0] - h->lb[0]; l.dx1 = h->ub[1] - h->lb[1];
+    l.m = lhs::half_bits((uint64_t)n_pool);
+    const int lgrid = (int)(blocks < 8LL * h->n_sm ? blocks : 8LL * h->n_sm);
+    lhs::draw_kernel<<<lgrid, lhs::THREADS, 0, h->stream>>>(l);
+    CUDA_TRY(cudaGetLastError());
+    h->launches++;
+    // its probe streams from the weights after every step already enqueued, as pinn_residual forms them
+    if (launch_forward_generic(h, px, pt, n_pool, 2, 4)) return -1;
+    rad::Args a{};
+    a.streams = h->d_pout; a.px = px; a.pt = pt;
+    a.a = pt + n_pool;
+    a.lp = reinterpret_cast<uint64_t*>(a.a + n_pool);
+    a.bmax = a.a + 2 * n_pool;
+    a.bsum = reinterpret_cast<uint64_t*>(a.bmax + rad::MAX_BLOCKS);
+    a.x = h->d_x + h->dcap; a.t = h->d_t + h->dcap;
+    a.n_pool = (uint64_t)n_pool; a.seg = (uint64_t)((n_pool + grid - 1) / grid); a.n = (uint64_t)n;
+    a.seed = seed; a.draw = draw; a.grid = grid;
+    a.nls = h->pde == PINN_NLS_INF; a.k = k; a.nu = h->nu; a.c = c;
+    rad::head_kernel<<<grid, rad::THREADS, 0, h->stream>>>(a);
+    CUDA_TRY(cudaGetLastError());
+    rad::quantise_kernel<<<grid, rad::THREADS, 0, h->stream>>>(a);
+    CUDA_TRY(cudaGetLastError());
+    const long long rows = (n + rad::THREADS - 1) / rad::THREADS;
+    rad::pick_kernel<<<(int)(rows < 8LL * h->n_sm ? rows : 8LL * h->n_sm), rad::THREADS, 0, h->stream>>>(a);
+    CUDA_TRY(cudaGetLastError());
+    h->launches += 3;
+  }
+  h->n_c = n; h->n_c_global = n;
+  h->map_x = h->map_t = nullptr;
   return 0;
 }
 
@@ -1437,20 +1503,10 @@ int pinn_lbfgs_history(pinn_t* h, double* f_hist_out, int capacity, int* n_out) 
   return 0;
 }
 
-// generic thread-per-point forward on host points (X != nullptr) or on a device SoA range (dx, dt)
-static int forward_generic(pinn_t* h, const double* X, const double* dx, const double* dt, int64_t n, int in_dim, double* out,
-                           int ns) {
-  if (!h || !out || (!X && !dx)) return fail("null argument");
-  if (n <= 0) return 0;
-  if (in_dim != 1 && in_dim != 2) return fail("in_dim must be 1 or 2");
-  CUDA_TRY(cudaSetDevice(h->device));
-  const int no = h->layers.back();
-  if (ensure(&h->d_pout, &h->pout_cap, n * no * ns)) return -1;
-  if (X) {
-    if (ensure(&h->d_px, &h->px_cap, n * in_dim)) return -1;
-    CUDA_TRY(cudaMemcpyAsync(h->d_px, X, n * in_dim * 8, cudaMemcpyHostToDevice, h->stream));
-    dx = h->d_px; dt = nullptr;
-  }
+// generic thread-per-point forward of n >= 1 device points into h->d_pout, [n][ns][no], enqueued on h->stream: interleaved
+// X[n][in_dim] in dx (dt == nullptr) or a SoA range (dx, dt)
+static int launch_forward_generic(pinn_t* h, const double* dx, const double* dt, int64_t n, int in_dim, int ns) {
+  if (ensure(&h->d_pout, &h->pout_cap, n * h->layers.back() * ns)) return -1;
   pinn::NetDesc nd = net_desc(h);
   const int threads = 64;
   const int blocks = (int)((n + threads - 1) / threads);
@@ -1467,7 +1523,23 @@ static int forward_generic(pinn_t* h, const double* X, const double* dx, const d
   }
   CUDA_TRY(cudaGetLastError());
   h->launches++;
-  CUDA_TRY(cudaMemcpyAsync(out, h->d_pout, n * no * ns * 8, cudaMemcpyDeviceToHost, h->stream));
+  return 0;
+}
+
+// generic thread-per-point forward on host points (X != nullptr) or on a device SoA range (dx, dt)
+static int forward_generic(pinn_t* h, const double* X, const double* dx, const double* dt, int64_t n, int in_dim, double* out,
+                           int ns) {
+  if (!h || !out || (!X && !dx)) return fail("null argument");
+  if (n <= 0) return 0;
+  if (in_dim != 1 && in_dim != 2) return fail("in_dim must be 1 or 2");
+  CUDA_TRY(cudaSetDevice(h->device));
+  if (X) {
+    if (ensure(&h->d_px, &h->px_cap, n * in_dim)) return -1;
+    CUDA_TRY(cudaMemcpyAsync(h->d_px, X, n * in_dim * 8, cudaMemcpyHostToDevice, h->stream));
+    dx = h->d_px; dt = nullptr;
+  }
+  if (launch_forward_generic(h, dx, dt, n, in_dim, ns)) return -1;
+  CUDA_TRY(cudaMemcpyAsync(out, h->d_pout, n * h->layers.back() * ns * 8, cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(cudaStreamSynchronize(h->stream));
   return 0;
 }

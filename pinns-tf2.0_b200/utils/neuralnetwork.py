@@ -143,6 +143,15 @@ class NeuralNetwork(object):
         # with e % resample_every == 0 the set is replaced by Latin-hypercube draw e // resample_every of resample_seed
         self.resample_every = _hp_int(hp, "resample_every", 0, 0)
         self.resample_seed = _hp_int(hp, "resample_seed", 0, 0, 1 << 64)
+        # optional residual-based adaptive resampling (not in the reference): before Adam epoch e > 0 with e % rad_every == 0 the
+        # set is replaced by RAD draw e // rad_every of resample_seed, N_f points from a pool of rad_pool (default 10 N_f) drawn
+        # with probability ~ |f|^rad_k / mean |f|^rad_k + rad_c at the current weights (pinn_draw_collocation_rad)
+        self.rad_every = _hp_int(hp, "rad_every", 0, 0)
+        self.rad_pool = None if _hp_get(hp, "rad_pool") is None else _hp_int(hp, "rad_pool", 1, 1, (1 << 29) + 1)
+        self.rad_k = _hp_int(hp, "rad_k", 1, 0, 5)
+        self.rad_c = _hp_real(hp, "rad_c", 1.0, 0.0, 1024.0)
+        if self.resample_every and self.rad_every:
+            raise pinn_cabi.PinnError('hp["resample_every"] and hp["rad_every"] both redraw the collocation set: set one of them')
         self._tf_epoch = 0
         self._h = None
         self._w0 = _glorot_normal(self.layers, np.random.default_rng(self.weight_seed))
@@ -208,6 +217,9 @@ class NeuralNetwork(object):
             pde = self._pde_id()
             if self.resample_every and pde not in _COLLOCATION:
                 raise pinn_cabi.PinnError('hp["resample_every"]: %s has no collocation set to resample' % type(self).__name__)
+            if self.rad_every and (pde not in _RAD or getattr(self, "world", 1) > 1):
+                raise pinn_cabi.PinnError('hp["rad_every"]: residual-based resampling runs for the Burgers and Schrodinger '
+                                          'inference models on one GPU, not for %s' % type(self).__name__)
             h = pinn_cabi.Pinn(pde, self.layers, self.lb, self.ub, device=getattr(self, "device", 0),
                                rank=getattr(self, "rank", 0), world=getattr(self, "world", 1),
                                nccl_uid=getattr(self, "nccl_uid", None))
@@ -345,9 +357,9 @@ class NeuralNetwork(object):
         return loss_and_flat_grad
 
     def tf_optimization(self, X_u, u):
-        """Adam epochs.  With hp["resample_every"] = k the collocation set is redrawn on the device before every epoch e > 0 with
-        e % k == 0 (tf_optimization_step); epochs [0, k) train on the script's own X_f, and the L-BFGS phase that follows runs on
-        the last drawn set."""
+        """Adam epochs.  With hp["resample_every"] = k (or hp["rad_every"] = k) the collocation set is redrawn on the device
+        before every epoch e > 0 with e % k == 0 (tf_optimization_step); epochs [0, k) train on the script's own X_f, and the
+        L-BFGS phase that follows runs on the last drawn set."""
         self.logger.log_train_opt("Adam")
         self._tf_epoch = 0
         for epoch in range(self.tf_epochs):
@@ -357,12 +369,16 @@ class NeuralNetwork(object):
     def tf_optimization_step(self, X_u, u):
         """One fused loss/grad evaluation + on-device Adam update, enqueued without a host sync.  With hp["resample_every"] = k,
         epoch e > 0 with e % k == 0 first replaces the collocation set by Latin-hypercube draw e // k of hp["resample_seed"] over
-        the script's N_f points (n_f_global when sharded), this rank's rows of it (pinn_draw_collocation)."""
+        the script's N_f points (n_f_global when sharded), this rank's rows of it (pinn_draw_collocation).  With
+        hp["rad_every"] = k the set becomes RAD draw e // k of hp["resample_seed"] instead (pinn_draw_collocation_rad)."""
         self._bind(X_u, u)
         n = self._native()
-        e, k = self._tf_epoch, self.resample_every
+        e, k, kr = self._tf_epoch, self.resample_every, self.rad_every
         if k and e > 0 and e % k == 0:
             self._resample(n, e // k)
+        if kr and e > 0 and e % kr == 0:
+            n_f = int(np.asarray(self.x_f).shape[0])
+            n.draw_collocation_rad(self.resample_seed, e // kr, n_f, self.rad_pool or 10 * n_f, self.rad_k, self.rad_c)
         self._tf_epoch = e + 1
         n.adam_step(self.tf_lr, self.tf_b1, self.tf_b2, self.tf_eps, sync=False)
         self._adam_serial = getattr(self, "_adam_serial", 0) + 1
@@ -422,15 +438,30 @@ _LAMBDAS = (pinn_cabi.BURGERS_IDE, pinn_cabi.NS_IDE, pinn_cabi.POLY_IDE) + _TWO_
 _POLY = (pinn_cabi.POLY_INF, pinn_cabi.POLY_IDE)
 # models with a collocation set (pinn_set_collocation, pinn_draw_collocation)
 _COLLOCATION = (pinn_cabi.BURGERS_INF, pinn_cabi.NLS_INF, pinn_cabi.POLY_INF)
+# models whose residual the device forms on a pool it has just drawn (pinn_draw_collocation_rad)
+_RAD = (pinn_cabi.BURGERS_INF, pinn_cabi.NLS_INF)
+
+
+def _hp_get(hp, key, default=None):
+    return hp.get(key, default) if hasattr(hp, "get") else default
 
 
 def _hp_int(hp, key, default, lo, hi=None):
     """An optional integer hyper-parameter in [lo, hi)."""
-    v = hp.get(key, default) if hasattr(hp, "get") else default
+    v = _hp_get(hp, key, default)
     v = default if v is None else v
     if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)) or v < lo or (hi is not None and v >= hi):
         raise pinn_cabi.PinnError('hp["%s"] = %r: expected an integer >= %d%s' % (key, v, lo, "" if hi is None else " below %d" % hi))
     return int(v)
+
+
+def _hp_real(hp, key, default, lo, hi):
+    """An optional finite real hyper-parameter in [lo, hi]."""
+    v = _hp_get(hp, key, default)
+    v = default if v is None else v
+    if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, float, np.integer, np.floating)) or not lo <= float(v) <= hi:
+        raise pinn_cabi.PinnError('hp["%s"] = %r: expected a real number in [%g, %g]' % (key, v, lo, hi))
+    return float(v)
 
 
 def _scalar(v):

@@ -46,6 +46,7 @@ SIGNATURES = {
     "pinn_set_collocation": (C.c_int, [C.c_void_p, _dp, _dp, C.c_int64, C.c_int64]),
     "pinn_set_collocation_mapped": (C.c_int, [C.c_void_p, _dp, _dp, C.c_int64, C.c_int64]),
     "pinn_draw_collocation": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, C.c_int64, C.c_int64, C.c_int64]),
+    "pinn_draw_collocation_rad": (C.c_int, [C.c_void_p, C.c_uint64, C.c_uint64, C.c_int64, C.c_int64, C.c_int, C.c_double]),
     "pinn_get_collocation": (C.c_int, [C.c_void_p, _dp, _dp, C.c_int64]),
     "pinn_set_data": (C.c_int, [C.c_void_p, _dp, C.c_int64, C.c_int, _dp, C.c_int, C.c_double]),
     "pinn_set_snapshot": (C.c_int, [C.c_void_p, C.c_int, _dp, C.c_int64, _dp]),
@@ -213,6 +214,15 @@ class Pinn(object):
                 raise PinnError(f"draw_collocation: {name} = {int(v)} is not an unsigned 64-bit integer")
         first, hi = shard_rows(int(n_global), int(rank), int(world))
         self._ck(self.lib.pinn_draw_collocation(self.h, int(seed), int(draw), first, hi - first, int(n_global)))
+
+    def draw_collocation_rad(self, seed, draw, n, n_pool, k=1, c=1.0):
+        """Replace the collocation set by n points drawn with replacement from Latin-hypercube draw `draw` of `seed` with n_pool
+        points, with probability ~ |f|^k / mean |f|^k + c at the current weights (residual-based adaptive resampling,
+        pinn_draw_collocation_rad).  Enqueued on the device; nothing is synchronised."""
+        for name, v in (("seed", seed), ("draw", draw)):
+            if not 0 <= int(v) < 1 << 64:
+                raise PinnError(f"draw_collocation_rad: {name} = {int(v)} is not an unsigned 64-bit integer")
+        self._ck(self.lib.pinn_draw_collocation_rad(self.h, int(seed), int(draw), int(n_pool), int(n), int(k), float(c)))
 
     def get_collocation(self):
         """(x, t) of the stored collocation set, however it got there (upload, mapped batch, draw)."""
