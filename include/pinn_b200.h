@@ -56,7 +56,8 @@ enum {
                            loss = sum (u - u_d)^2 + sum (v - v_d)^2 + sum f_u^2 + sum f_v^2 over the data points (parts: data, 0,
                            residual); flat vector ends with the raw [lambda_1, lambda_2]; one GPU only (world == 1)          */,
   PINN_POLY_INF = 8,    /* user-defined residual (pinn_set_residual) on a net [2, ..., 1]:
-                           f = sum_k c_k kappa_k u^a_k u_x^b_k u_t^c_k u_xx^d_k - s(x, t); every kappa_k = 1;
+                           f = sum_k c_k kappa_k u^a_k u_x^b_k u_t^c_k u_xx^d_k - s(x, t); every kappa_k = 1; s is an
+                           array (pinn_set_source) or a table the device evaluates (pinn_set_source_terms);
                            loss structure of BURGERS_INF (data term of pinn_set_data + mean f^2 over pinn_set_collocation)  */
   PINN_POLY_IDE = 9     /* as POLY_INF with kappa_k in {1, l1, l2, e^l1, e^l2}; loss structure of BURGERS_IDE (the residual on the
                            data points); flat vector ends with the raw [lambda_1, lambda_2].  Both poly ids run on the generic
@@ -134,12 +135,13 @@ int pinn_set_collocation_mapped(pinn_t* h, const double* x_pinned, const double*
  * of `seed` over [lb, ub] of pinn_create, with N = n_global strata per dimension (DESIGN §4.6).  Enqueue only: no host buffer,
  * no synchronisation (except when the collocation region has to grow, as for pinn_set_collocation).  n_global is also the MSE_f
  * denominator, as in pinn_set_collocation; 1 <= n_global <= 2^53 and 0 <= first <= first + n <= n_global.  Replaces a mapped
- * batch.  POLY_INF: the source resets to zero, like every new set of residual points.  The drawn set is a current input of the
+ * batch.  POLY_INF: an array source resets to zero and a source table is evaluated at the new set, as for every new set of
+ * residual points.  The drawn set is a current input of the
  * handle, defined by (seed, draw, first, n, n_global, lb, ub): the handle equals a fresh one fed the same points through
  * pinn_set_collocation.  The row rule: one Philox4x32-10 block of (row, draw) under the seed gives two 53-bit uniforms, two
  * keyed Feistel permutations of [0, n_global) give the strata, and x_d = lb_d + (ub_d - lb_d) * ((stratum + u) / n_global). */
 int pinn_draw_collocation(pinn_t* h, uint64_t seed, uint64_t draw, int64_t first, int64_t n, int64_t n_global);
-/* BURGERS_INF, NLS_INF, one GPU: residual-based adaptive resampling (RAD, Wu et al., CMAME 403, 2023; DESIGN §4.7).  Replaces
+/* BURGERS_INF, NLS_INF, POLY_INF, one GPU: residual-based adaptive resampling (RAD, Wu et al., CMAME 403, 2023; DESIGN §4.7).  Replaces
  * the collocation set by n points drawn, with replacement, from a pool with probability proportional to a quantised
  * eps(x)^k / E[eps^k] + c, where eps is the PDE residual at the handle's current weights.  Enqueue only, like
  * pinn_draw_collocation: no host buffer, no synchronisation (except when the collocation region or the pool scratch has to grow).
@@ -148,7 +150,7 @@ int pinn_draw_collocation(pinn_t* h, uint64_t seed, uint64_t draw, int64_t first
  *   1. pool: rows [0, n_pool) of Latin-hypercube draw `draw` of `seed` with n_pool strata, i.e. what
  *      pinn_draw_collocation(h, seed, draw, 0, n_pool, n_pool) stores;
  *   2. f_i at pool point i, from the weights after every step already enqueued: bit for bit the value pinn_residual returns;
- *   3. r_i = |f_i| (BURGERS_INF) or sqrt(f_u^2 + f_v^2) (NLS_INF), each operation rounded; a_i = r_i^k as left-to-right rounded
+ *   3. r_i = |f_i| (BURGERS_INF, POLY_INF) or sqrt(f_u^2 + f_v^2) (NLS_INF), each operation rounded; a_i = r_i^k as left-to-right rounded
  *      products (k = 0: a_i = 1);
  *   4. amax = the largest finite a_i (0 if none); A_i = 2^24 if a_i is not finite, else floor((a_i / amax) * 2^24) as a uint64
  *      (0 when amax = 0); S = sum A_i; C' = floor(c * (double)S / n_pool) (one rounded fp64 multiply, one rounded divide);
@@ -158,12 +160,15 @@ int pinn_draw_collocation(pinn_t* h, uint64_t seed, uint64_t draw, int64_t first
  *      the least i whose inclusive prefix Q_0 + ... + Q_i exceeds target.
  * Points with Q_i = 0 are never drawn; a non-finite residual takes the largest weight.  Up to the 2^-24 quantisation Q_i / T is
  * RAD's (a_i / mean a + c) / (n_pool (1 + c)).  Unlike Wu et al. the draw is with replacement: a point may appear more than once.
- * Refused (the handle is left unchanged) for the identification, discrete-time and Navier-Stokes models, for POLY_INF (its
- * source lives on the host), for world > 1, and unless 0 <= k <= 4, c is finite in [0, 1024], 1 <= n_pool <= 2^29 and n >= 0. */
+ * POLY_INF: f is the residual spec's sum in pinn_residual's order, each product and sum rounded, minus the source table's s at
+ * the pool point; the table is then evaluated at the drawn set.  Refused (the handle is left unchanged) for the identification,
+ * discrete-time and Navier-Stokes models, for POLY_INF without a residual spec or with an array source (pinn_set_source: values
+ * at the stored points say nothing about a pool), for world > 1, and unless 0 <= k <= 4, c is finite in [0, 1024],
+ * 1 <= n_pool <= 2^29 and n >= 0. */
 int pinn_draw_collocation_rad(pinn_t* h, uint64_t seed, uint64_t draw, int64_t n_pool, int64_t n, int k, double c);
 /* The stored collocation set, however it got there (upload, mapped batch, draw): x, t hold n doubles each; n must equal
- * pinn_num_residual_points(h).  Synchronises.  A POLY_INF caller with a source reads a drawn set back here, evaluates s(x, t)
- * and calls pinn_set_source. */
+ * pinn_num_residual_points(h).  Synchronises.  (A POLY_INF source that a table cannot express is evaluated on a set read back
+ * here and stored with pinn_set_source.) */
 int pinn_get_collocation(pinn_t* h, double* x, double* t, int64_t n);
 
 /* Data term: X_u,u of fit(X_u,u) (utils/neuralnetwork.py:138-146).  X is (n,in_dim) row-major; in_dim==1
@@ -185,9 +190,29 @@ int pinn_set_snapshot(pinn_t* h, int which, const double* x, int64_t n, const do
  * spec may be replaced at any time; evaluating a poly handle before it is set is an error. */
 int pinn_set_residual(pinn_t* h, int n_terms, const double* coef, const int* kind, const int* exps);
 /* POLY_INF / POLY_IDE: the source s at the stored residual points, n == pinn_num_residual_points(h).  Storing new residual
- * points (pinn_set_collocation for POLY_INF, pinn_set_data for POLY_IDE) resets the source to zero, so a source never
- * outlives the points it was computed for. */
+ * points (pinn_set_collocation, pinn_draw_collocation and pinn_draw_collocation_rad for POLY_INF, pinn_set_data for POLY_IDE)
+ * resets the source to zero, so a source never outlives the points it was computed for.  Removes a source table. */
 int pinn_set_source(pinn_t* h, const double* s, int64_t n);
+/* POLY_INF / POLY_IDE: the source as a function the device evaluates (DESIGN §4.8), a sum of n_terms separable terms
+ *   s(x, t) = sum_k a_k x^p_k t^q_k X_k(x) T_k(t) exp(alpha_k x + gamma_k x^2 + beta_k t + delta_k t^2),
+ * X_k one of 1, sin(omega_k x + phi_k), cos(omega_k x + phi_k) and T_k one of 1, sin(nu_k t + psi_k), cos(nu_k t + psi_k).
+ * form[k] = p_k | q_k << 2 | xkind_k << 4 | tkind_k << 6 with p, q in 0..3 and the kinds 0: 1, 1: sin, 2: cos; par is
+ * n_terms x 9 row-major (a, omega, phi, nu, psi, alpha, gamma, beta, delta), every entry finite; 0 <= n_terms <= 16.  A refused
+ * call changes nothing.  Evaluation order, every product and sum rounded on its own (no contraction):
+ *   m = a; m *= x, p times; m *= t, q times; m *= X(omega * x + phi); m *= T(nu * t + psi);
+ *   m *= exp(((alpha * x + gamma * (x * x)) + beta * t) + delta * (t * t)), omitted when alpha, gamma, beta and delta are all 0;
+ *   s = ((0 + m_0) + m_1) + ... in term order.
+ * exp is CUDA's exp; sin and cos are CUDA's sin and cos for arguments of magnitude below 2^31 (the library's fast path,
+ * restated bit for bit) and NaN from 2^31 on.  Non-finite x or t propagate into s.  A table is a function and follows the
+ * points: setting it evaluates it at the stored residual points, and every new set of residual points (pinn_set_collocation,
+ * pinn_draw_collocation, pinn_draw_collocation_rad for POLY_INF; pinn_set_data for POLY_IDE) is evaluated again, enqueued
+ * (only a growing source array synchronises).  Setting a table removes an array source (pinn_set_source) and vice versa;
+ * n_terms = 0 removes both.  A handle with a table equals a fresh one fed the same points and pinn_set_source of
+ * pinn_get_source. */
+int pinn_set_source_terms(pinn_t* h, int n_terms, const int* form, const double* par);
+/* POLY_INF / POLY_IDE: the stored source at the residual points, however it was formed (array, table or none: zeros);
+ * n == pinn_num_residual_points(h).  Synchronises. */
+int pinn_get_source(pinn_t* h, double* s, int64_t n);
 
 /* NLS periodic-boundary times tb (N_b,1): X_lb=(lb0,tb), X_ub=(ub0,tb) (inf_cont_schrodinger.py:50-53).
  * BURGERS_DISC: the boundary positions x_1 on which sum(net(x_1)^2) is imposed (inf_disc_burgers.py:57,99). */

@@ -13,7 +13,7 @@ LIB_DIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIB_DIR, "libpinn_b200.so")
 SOURCES = ["pinn_api.cu"]
 HEADERS = ["pinn_common.cuh", "burgers_fused.cuh", "burgers_fused_v2.cuh", "nls_fused.cuh", "generic_fused.cuh", "optim_kernels.cuh",
-           "navier_stokes_fused.cuh", "lhs_draw.cuh", "rad_sample.cuh",
+           "navier_stokes_fused.cuh", "lhs_draw.cuh", "rad_sample.cuh", "source_terms.cuh",
            os.path.join("..", "..", "include", "pinn_b200.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]

@@ -20,6 +20,7 @@
 #include "navier_stokes_fused.cuh"
 #include "lhs_draw.cuh"
 #include "rad_sample.cuh"
+#include "source_terms.cuh"
 
 namespace {
 
@@ -295,9 +296,12 @@ struct pinn_handle {
   double* d_rad = nullptr;                  // pinn_draw_collocation_rad: pool x, t, r^k, segment prefixes, block maxima and sums
   long long rad_cap = 0;
 
-  // POLY_INF / POLY_IDE: the residual's term table (n == 0: not set yet) and the source at the residual points (empty: 0)
+  // POLY_INF / POLY_IDE: the residual's term table (n == 0: not set yet) and the source: an array of values at the residual
+  // points (h_src, copied to d_src; empty: none) or a table the device evaluates into d_src at every new set of points
+  // (src_tab.n == 0: none).  At most one of the two is set.
   pinn::generic::PolySpec poly{};
   std::vector<double> h_src;
+  pinn::source::Table src_tab{};
   double* d_src = nullptr;
   long long src_cap = 0;
 
@@ -496,6 +500,22 @@ int upload(pinn_t* h, double** p, long long* cap, const double* src, long long n
   return 0;
 }
 
+// POLY_INF / POLY_IDE with a source table: enqueues s at the stored residual points into d_src (the collocation set, or the
+// data points for POLY_IDE).  Called whenever those points or the table change; only a growing d_src synchronises.
+int fill_source(pinn_t* h) {
+  const long long n = pinn_num_residual_points(h);
+  if (h->src_tab.n == 0 || n == 0) return 0;
+  if (ensure(&h->d_src, &h->src_cap, n)) return -1;
+  const long long off = model(h).residual == Res::Data ? h->dcap - h->n_d : h->dcap;
+  const long long blocks = (n + pinn::source::THREADS - 1) / pinn::source::THREADS;
+  const int grid = (int)(blocks < 8LL * h->n_sm ? blocks : 8LL * h->n_sm);     // one wave of 256-thread blocks, grid-stride beyond
+  pinn::source::eval_kernel<<<grid, pinn::source::THREADS, 0, h->stream>>>(h->src_tab, h->d_x + off, h->d_t + off, h->d_src,
+                                                                            (uint64_t)n);
+  CUDA_TRY(cudaGetLastError());
+  h->launches++;
+  return 0;
+}
+
 // Records h's most recent fused launch for the tail that reduces it (make_tail, launch_tail): the grid, the stride of the
 // partial vectors and the ReduceMap -- the p_net net-gradient entries, then the partial-vector entries of the two trained lambdas
 // (lam; nullptr when there are none) and of the data, boundary and residual loss parts.
@@ -683,7 +703,7 @@ int generic_launch_eval(pinn_t* h, const int* run_flag) {
   a.partials = h->d_partials; a.pstride = h->pstride; a.run_flag = run_flag;
   if (m.poly) {
     a.poly = h->poly;
-    a.src = h->h_src.empty() ? nullptr : h->d_src;
+    a.src = h->h_src.empty() && h->src_tab.n == 0 ? nullptr : h->d_src;
     G::fused_loss_grad<true><<<grid, G::THREADS, 0, h->stream>>>(a);
   } else {
     G::fused_loss_grad<false><<<grid, G::THREADS, 0, h->stream>>>(a);
@@ -1111,8 +1131,8 @@ int pinn_set_collocation(pinn_t* h, const double* x, const double* t, int64_t n,
   }
   h->n_c = n; h->n_c_global = n_global;
   h->map_x = h->map_t = nullptr;
-  h->h_src.clear();                               // POLY_INF: new residual points, the source is 0 until set again
-  return 0;
+  h->h_src.clear();                               // POLY_INF: new residual points, an array source is 0 until set again
+  return fill_source(h);                          // ... and a table follows them
 }
 
 int pinn_draw_collocation(pinn_t* h, uint64_t seed, uint64_t draw, int64_t first, int64_t n, int64_t n_global) {
@@ -1140,8 +1160,8 @@ int pinn_draw_collocation(pinn_t* h, uint64_t seed, uint64_t draw, int64_t first
   }
   h->n_c = n; h->n_c_global = n_global;
   h->map_x = h->map_t = nullptr;
-  h->h_src.clear();                               // POLY_INF: new residual points, the source is 0 until set again
-  return 0;
+  h->h_src.clear();                               // POLY_INF: new residual points, an array source is 0 until set again
+  return fill_source(h);                          // ... and a table follows them
 }
 
 static int launch_forward_generic(pinn_t* h, const double* dx, const double* dt, int64_t n, int in_dim, int ns);
@@ -1153,9 +1173,11 @@ int pinn_draw_collocation_rad(pinn_t* h, uint64_t seed, uint64_t draw, int64_t n
     return fail("pinn_draw_collocation_rad: identification uses the data points as residual points");
   if (m.residual == Res::None)
     return fail("pinn_draw_collocation_rad: the discrete-time models have no collocation set (snapshot / boundary points only)");
-  if (m.poly)
-    return fail("pinn_draw_collocation_rad: POLY_INF's source s(x, t) lives on the host, so its residual cannot be formed on a "
-                "pool drawn on the device");
+  if (m.poly && h->poly.n == 0)
+    return fail("pinn_draw_collocation_rad: POLY_INF has no residual spec to weight the pool by (call pinn_set_residual first)");
+  if (m.poly && !h->h_src.empty())
+    return fail("pinn_draw_collocation_rad: POLY_INF's source is an array of values at the stored points, which says nothing about "
+                "a pool drawn on the device; give it as a table the device evaluates (pinn_set_source_terms)");
   if (h->world > 1)
     return fail("pinn_draw_collocation_rad: runs on one GPU (world must be 1): the weights are normalised over the whole pool");
   if (k < 0 || k > 4) return fail("pinn_draw_collocation_rad: k must be in 0..4");
@@ -1193,7 +1215,13 @@ int pinn_draw_collocation_rad(pinn_t* h, uint64_t seed, uint64_t draw, int64_t n
     a.n_pool = (uint64_t)n_pool; a.seg = (uint64_t)((n_pool + grid - 1) / grid); a.n = (uint64_t)n;
     a.seed = seed; a.draw = draw; a.grid = grid;
     a.nls = h->pde == PINN_NLS_INF; a.k = k; a.nu = h->nu; a.c = c;
-    rad::head_kernel<<<grid, rad::THREADS, 0, h->stream>>>(a);
+    if (m.poly) {
+      // f of the residual spec minus the table's s at every pool point (source_terms.cuh)
+      source::PoolArgs pa{a, h->poly, h->src_tab};
+      source::pool_head_kernel<<<grid, source::THREADS, 0, h->stream>>>(pa);
+    } else {
+      rad::head_kernel<<<grid, rad::THREADS, 0, h->stream>>>(a);
+    }
     CUDA_TRY(cudaGetLastError());
     rad::quantise_kernel<<<grid, rad::THREADS, 0, h->stream>>>(a);
     CUDA_TRY(cudaGetLastError());
@@ -1204,7 +1232,7 @@ int pinn_draw_collocation_rad(pinn_t* h, uint64_t seed, uint64_t draw, int64_t n
   }
   h->n_c = n; h->n_c_global = n;
   h->map_x = h->map_t = nullptr;
-  return 0;
+  return fill_source(h);                          // POLY_INF: the table follows the new set
 }
 
 int pinn_get_collocation(pinn_t* h, double* x, double* t, int64_t n) {
@@ -1282,8 +1310,9 @@ int pinn_set_data(pinn_t* h, const double* X, int64_t n, int in_dim, const doubl
   if (m.boundary) return assemble_points(h);
   // shrinking/growing the data set moves its right-aligned start; the collocation region is untouched
   if (upload_points(h)) return -1;
-  if (m.residual == Res::Data) h->h_src.clear();   // new residual points: the source is 0 until set again
-  return 0;
+  if (m.residual != Res::Data) return 0;
+  h->h_src.clear();                                // new residual points: an array source is 0 until set again
+  return fill_source(h);                           // ... and a table follows them
 }
 
 int pinn_set_residual(pinn_t* h, int n_terms, const double* coef, const int* kind, const int* exps) {
@@ -1326,6 +1355,54 @@ int pinn_set_source(pinn_t* h, const double* src, int64_t n) {
   CUDA_TRY(cudaSetDevice(h->device));
   if (upload(h, &h->d_src, &h->src_cap, src, n)) return -1;
   h->h_src.assign(src, src + n);
+  h->src_tab.n = 0;                               // an array replaces a table
+  return 0;
+}
+
+int pinn_set_source_terms(pinn_t* h, int n_terms, const int* form, const double* par) {
+  namespace S = pinn::source;
+  if (!h) return fail("null handle");
+  if (!model(h).poly)
+    return fail("pinn_set_source_terms: only the polynomial residual models (POLY_INF, POLY_IDE) take a source");
+  if (n_terms < 0 || n_terms > S::MAXT)
+    return fail("pinn_set_source_terms: n_terms = " + std::to_string(n_terms) + " is outside 0..16");
+  if (n_terms > 0 && (!form || !par)) return fail("pinn_set_source_terms: null argument");
+  static const char* const PAR[S::NPAR] = {"a", "omega", "phi", "nu", "psi", "alpha", "gamma", "beta", "delta"};
+  S::Table tb{};
+  tb.n = n_terms;
+  for (int k = 0; k < n_terms; k++) {
+    const std::string term = "pinn_set_source_terms: term " + std::to_string(k) + ": ";
+    const int f = form[k];
+    if (f < 0 || f > 255) return fail(term + "form " + std::to_string(f) + " is outside 0..255 (p | q << 2 | X kind << 4 | T kind << 6)");
+    if (((f >> 4) & 3) == 3) return fail(term + "X kind 3 is outside 0..2 (1, sin, cos)");
+    if (((f >> 6) & 3) == 3) return fail(term + "T kind 3 is outside 0..2 (1, sin, cos)");
+    tb.form[k] = f;
+    for (int j = 0; j < S::NPAR; j++) {
+      const double v = par[S::NPAR * k + j];
+      if (!std::isfinite(v)) return fail(term + "parameter " + PAR[j] + " is not finite");
+      tb.par[S::NPAR * k + j] = v;
+    }
+  }
+  CUDA_TRY(cudaSetDevice(h->device));
+  h->h_src.clear();                               // a table replaces an array
+  h->src_tab = tb;
+  return fill_source(h);
+}
+
+int pinn_get_source(pinn_t* h, double* s, int64_t n) {
+  if (!h) return fail("null handle");
+  if (!model(h).poly) return fail("pinn_get_source: only the polynomial residual models (POLY_INF, POLY_IDE) have a source");
+  const int64_t want = pinn_num_residual_points(h);
+  if (n != want)
+    return fail("pinn_get_source: the output buffer holds " + std::to_string(n) + " values but " + std::to_string(want) +
+                " residual points are stored (pinn_num_residual_points)");
+  if (n == 0) return 0;
+  if (!s) return fail("pinn_get_source: null argument");
+  CUDA_TRY(cudaSetDevice(h->device));
+  if (h->src_tab.n) CUDA_TRY(cudaMemcpyAsync(s, h->d_src, (size_t)n * 8, cudaMemcpyDeviceToHost, h->stream));
+  else if (!h->h_src.empty()) memcpy(s, h->h_src.data(), (size_t)n * 8);
+  else for (int64_t i = 0; i < n; i++) s[i] = 0.0;
+  CUDA_TRY(cudaStreamSynchronize(h->stream));
   return 0;
 }
 
@@ -1608,6 +1685,12 @@ int pinn_residual(pinn_t* h, double* f_out, int64_t n_rows) {
   }
   if (poly) {
     // the kernel head's f, term by term on the host: sum_k c_k kappa_k prod_j v_j^e_kj - s
+    std::vector<double> tab_src;
+    if (h->src_tab.n) {
+      tab_src.resize(n);
+      if (pinn_get_source(h, tab_src.data(), n)) return -1;
+    }
+    const double* src = h->src_tab.n ? tab_src.data() : h->h_src.empty() ? nullptr : h->h_src.data();
     double lam[2] = {0.0, 0.0};
     if (ide) CUDA_TRY(cudaMemcpy(lam, h->d_w + h->P_net, 16, cudaMemcpyDeviceToHost));
     const double kv[5] = {1.0, lam[0], lam[1], std::exp(lam[0]), std::exp(lam[1])};
@@ -1621,7 +1704,7 @@ int pinn_residual(pinn_t* h, double* f_out, int64_t n_rows) {
           for (int e = (code >> (3 + 2 * j)) & 3; e > 0; e--) m *= d[j];
         f += kv[code & 7] * m;
       }
-      f_out[i] = h->h_src.empty() ? f : f - h->h_src[i];
+      f_out[i] = src ? f - src[i] : f;
     }
     return 0;
   }

@@ -95,7 +95,9 @@ class NeuralNetwork(object):
     #                      | "kdv_ide_disc" | "ac_disc" | "ns_ide" | "poly" (the last four are never guessed from attributes)
     residual = None      # pde = "poly": the residual as a string, e.g. "u_t + u*u_x - nu*u_xx" (utils/poly_spec.py); a spec that
     #                      mentions l1 / l2 is identification (fit(X_u, u), residual on the data points), otherwise inference
-    #                      (collocation x_f, t_f).  An optional method source(x, t) gives s in f = ... - s.
+    #                      (collocation x_f, t_f).  An optional source gives s in f = ... - s: a string such as
+    #                      "(k*pi**2 - 1)*sin(pi*x)*exp(-t)" (poly_spec.parse_source), which the device evaluates at every new set of
+    #                      points, or a method source(x, t), evaluated on the host whenever the points change.
     weight_seed = 1234   # stands in for tf.random.set_seed(1234) (inf_cont_burgers.py:10)
 
     def __init_subclass__(cls, **kw):
@@ -183,23 +185,37 @@ class NeuralNetwork(object):
                 "burgers_disc": pinn_cabi.BURGERS_DISC, "burgers_ide_disc": pinn_cabi.BURGERS_IDE_DISC,
                 "kdv_ide_disc": pinn_cabi.KDV_IDE_DISC, "ac_disc": pinn_cabi.AC_DISC, "ns_ide": pinn_cabi.NS_IDE}[tag]
 
+    def _resolve_name(self, name):
+        """The number a free name of a residual or source string stands for: a numeric attribute of the instance, else None."""
+        v = getattr(self, name, None)
+        if isinstance(v, (bool, np.bool_, str, bytes)) or v is None or callable(v):
+            return None
+        try:
+            a = np.asarray(v, dtype=np.float64)
+        except (TypeError, ValueError):
+            return None
+        return float(a.reshape(-1)[0]) if a.size == 1 else None
+
     def _poly_spec(self):
         """The parsed `residual` string (pde = "poly"); free names resolve to numeric attributes of the instance."""
         if getattr(self, "_poly_cache", None) is None:
-            def resolve(name):
-                v = getattr(self, name, None)
-                if isinstance(v, (bool, np.bool_, str, bytes)) or v is None or callable(v):
-                    return None
-                try:
-                    a = np.asarray(v, dtype=np.float64)
-                except (TypeError, ValueError):
-                    return None
-                return float(a.reshape(-1)[0]) if a.size == 1 else None
             try:
-                self._poly_cache = poly_spec.parse(self.residual, resolve)
+                self._poly_cache = poly_spec.parse(self.residual, self._resolve_name)
             except poly_spec.SpecError as e:
                 raise pinn_cabi.PinnError("%s.residual: %s" % (type(self).__name__, e))
         return self._poly_cache
+
+    def _source_table(self):
+        """The parsed `source` string (pde = "poly"); free names resolve as in the residual.  A table whose exp factor overflows
+        on the box [lb, ub] is refused."""
+        if getattr(self, "_source_cache", None) is None:
+            try:
+                terms = poly_spec.parse_source(self.source, self._resolve_name)
+                poly_spec.check_source_range(terms, self.lb, self.ub)
+                self._source_cache = terms
+            except poly_spec.SpecError as e:
+                raise pinn_cabi.PinnError("%s.source: %s" % (type(self).__name__, e))
+        return self._source_cache
 
     def _upload_source(self, X, h=None):
         """pde = "poly": source(x, t) on the residual points X (N, 2) just bound, when the subclass defines it."""
@@ -217,9 +233,11 @@ class NeuralNetwork(object):
             pde = self._pde_id()
             if self.resample_every and pde not in _COLLOCATION:
                 raise pinn_cabi.PinnError('hp["resample_every"]: %s has no collocation set to resample' % type(self).__name__)
-            if self.rad_every and (pde not in _RAD or getattr(self, "world", 1) > 1):
+            rad_ok = pde in _RAD or (pde == pinn_cabi.POLY_INF and isinstance(getattr(self, "source", None), str))
+            if self.rad_every and (not rad_ok or getattr(self, "world", 1) > 1):
                 raise pinn_cabi.PinnError('hp["rad_every"]: residual-based resampling runs for the Burgers and Schrodinger '
-                                          'inference models on one GPU, not for %s' % type(self).__name__)
+                                          'inference models and for poly inference with a string source (use "0" for none) on '
+                                          'one GPU, not for %s' % type(self).__name__)
             h = pinn_cabi.Pinn(pde, self.layers, self.lb, self.ub, device=getattr(self, "device", 0),
                                rank=getattr(self, "rank", 0), world=getattr(self, "world", 1),
                                nccl_uid=getattr(self, "nccl_uid", None))
@@ -243,6 +261,8 @@ class NeuralNetwork(object):
                 w = np.concatenate([w, [_scalar(getattr(self, "lambda_1", 0.0)), _scalar(getattr(self, "lambda_2", 0.0))]])
             elif pde in _POLY:                                       # utils/poly_spec.py
                 h.set_residual(self._poly_spec().terms)
+                if isinstance(getattr(self, "source", None), str):   # a table: it follows every new set of residual points
+                    h.set_source_terms(self._source_table())
                 if pde == pinn_cabi.POLY_IDE:                        # raw lambdas, 0.0 unless the class sets them
                     w = np.concatenate([w, [_scalar(getattr(self, "lambda_1", 0.0)), _scalar(getattr(self, "lambda_2", 0.0))]])
                 else:
@@ -388,7 +408,7 @@ class NeuralNetwork(object):
         n_global = getattr(self, "n_f_global", None) or int(np.asarray(self.x_f).shape[0])
         n.draw_collocation(self.resample_seed, draw, n_global, rank=getattr(self, "rank", 0), world=getattr(self, "world", 1))
         if n.pde == pinn_cabi.POLY_INF and callable(getattr(self, "source", None)):
-            x, t = n.get_collocation()                       # the one host round trip a source needs
+            x, t = n.get_collocation()                       # the one host round trip a callable source needs
             self._upload_source(np.stack([x, t], 1), n)
 
     def nt_optimization(self, X_u, u):
@@ -501,7 +521,9 @@ def _native_f_model(self, *args):
             lam = n.get_weights()[-2:] if n.pde == pinn_cabi.POLY_IDE else (0.0, 0.0)
             f = poly_spec.evaluate(self._poly_spec().terms, (U, Ux, Ut, Uxx), *lam)
             fn = getattr(self, "source", None)
-            if callable(fn):
+            if isinstance(fn, str):
+                f = f - poly_spec.evaluate_source(self._source_table(), X[:, 0:1], X[:, 1:2]).reshape(f.shape)
+            elif callable(fn):
                 f = f - np.asarray(fn(X[:, 0:1], X[:, 1:2]), dtype=np.float64).reshape(f.shape)
             return _t(f)
         if n.pde == pinn_cabi.POLY_IDE and self._bound is None:

@@ -20,6 +20,9 @@ BURGERS_INF, BURGERS_IDE, NLS_INF, BURGERS_DISC, BURGERS_IDE_DISC, KDV_IDE_DISC,
 POLY_INF, POLY_IDE = 8, 9
 # kappa_k of a polynomial residual term, in the order of pinn_set_residual's kind
 POLY_KINDS = ("1", "l1", "l2", "exp(l1)", "exp(l2)")
+# X_k and T_k of a source-table term, in the order of pinn_set_source_terms' kinds
+SOURCE_KINDS = ("1", "sin", "cos")
+SOURCE_MAXT = 16
 # Navier-Stokes derivative streams, in the order of pinn_derivatives' blocks
 NS_STREAMS = ("u", "x", "y", "t", "xx", "xy", "yy", "xt", "yt", "xxx", "xxy", "xyy", "yyy")
 LBFGS_REASONS = {0: "running", 1: "max iterations", 2: "max evaluations", 3: "optimality", 4: "step below tolX",
@@ -53,6 +56,8 @@ SIGNATURES = {
     "pinn_set_boundary": (C.c_int, [C.c_void_p, _dp, C.c_int64]),
     "pinn_set_residual": (C.c_int, [C.c_void_p, C.c_int, _dp, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "pinn_set_source": (C.c_int, [C.c_void_p, _dp, C.c_int64]),
+    "pinn_set_source_terms": (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_int), _dp]),
+    "pinn_get_source": (C.c_int, [C.c_void_p, _dp, C.c_int64]),
     "pinn_set_weights": (C.c_int, [C.c_void_p, _dp, C.c_int64]),
     "pinn_get_weights": (C.c_int, [C.c_void_p, _dp, C.c_int64]),
     "pinn_loss_grad": (C.c_int, [C.c_void_p, _dp, _dp, _dp, _dp]),
@@ -260,6 +265,19 @@ class Pinn(object):
         s = _arr(s).reshape(-1)
         self._ck(self.lib.pinn_set_source(self.h, _p(s), s.size))
 
+    def set_source_terms(self, terms):
+        """POLY_INF / POLY_IDE: the source as a table the device evaluates at every new set of residual points (see
+        pack_source_terms); an empty table removes the source."""
+        form, par = pack_source_terms(terms)
+        fp = form.ctypes.data_as(C.POINTER(C.c_int))
+        self._ck(self.lib.pinn_set_source_terms(self.h, len(form), fp, _p(par)))
+
+    def get_source(self):
+        """The stored source at the residual points, however it was formed (array, table, or zeros without a source)."""
+        s = np.empty(int(self.lib.pinn_num_residual_points(self.h)))
+        self._ck(self.lib.pinn_get_source(self.h, _p(s), s.size))
+        return s
+
     # ---- parameters
     def set_weights(self, w):
         w = _arr(w).reshape(-1)
@@ -429,6 +447,31 @@ class Lbfgs(object):
             self.close()
         except Exception:
             pass
+
+
+def pack_source_terms(terms):
+    """Source-table terms (a, p, q, xkind, omega, phi, tkind, nu, psi, alpha, gamma, beta, delta) -> (form, par) of
+    pinn_set_source_terms, with its checks: at most 16 terms, p and q in 0..3, kinds in 0..2 (SOURCE_KINDS), every parameter
+    finite."""
+    terms = [tuple(t) for t in terms]
+    if len(terms) > SOURCE_MAXT:
+        raise PinnError(f"set_source_terms: {len(terms)} terms; at most {SOURCE_MAXT} are supported")
+    form = np.zeros(max(len(terms), 1), dtype=np.intc)
+    par = np.zeros((max(len(terms), 1), 9))
+    for k, t in enumerate(terms):
+        if len(t) != 13:
+            raise PinnError(f"set_source_terms: term {k} has {len(t)} entries, expected 13 "
+                            "(a, p, q, xkind, omega, phi, tkind, nu, psi, alpha, gamma, beta, delta)")
+        a, p, q, xk, om, ph, tk, nu, ps, al, ga, be, de = t
+        for name, v, hi in (("p", p, 3), ("q", q, 3), ("xkind", xk, 2), ("tkind", tk, 2)):
+            if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)) or not 0 <= v <= hi:
+                raise PinnError(f"set_source_terms: term {k}: {name} = {v!r} is outside 0..{hi}")
+        for name, v in zip(("a", "omega", "phi", "nu", "psi", "alpha", "gamma", "beta", "delta"), (a, om, ph, nu, ps, al, ga, be, de)):
+            if not np.isfinite(float(v)):
+                raise PinnError(f"set_source_terms: term {k}: parameter {name} is not finite")
+        form[k] = int(p) | int(q) << 2 | int(xk) << 4 | int(tk) << 6
+        par[k] = (a, om, ph, nu, ps, al, ga, be, de)
+    return form[:len(terms)], par[:len(terms)]
 
 
 def irk_ide_disc(IRK_alpha, IRK_beta):
